@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the ngp_pl hot path on B200 (BASELINE.json metric: training rays/s,
+"""bench.py -- headline benchmark of the ngp_pl hot path on H100 (BASELINE.json metric: training rays/s,
 plus 800x800 render FPS), one JSON line on rank 0.
 
-    python bench.py --gpus 1 --steps K --warmup W            # this repo's sm_100a path
+    python bench.py --gpus 1 --steps K --warmup W            # this repo's sm_90a path
     python bench.py --impl reference ...                     # the reference's own path, same config
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...   # N ranks, one per GPU
     python bench.py --workload c5 ...                        # BASELINE config 5 (unbounded, 6 cascades, 4096 rays)
@@ -64,6 +64,10 @@ def parse():
     ap.add_argument("--no-fps", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-vren-ops", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, take ONE more step of the timed path (same captured graphs) from the seeded "
+                         "initial state -- not one of the timed steps, whose state is not reproducible -- and write what it "
+                         "computes as DIR/<name>.npy (float32): render, loss terms, the whole gradient")
     ap.add_argument("--ref-tcnn", default="fast", choices=["fast", "standin"],
                     help="--impl reference: which tinycudann stand-in drives the reference's Python (fast = performance-grade)")
     ap.add_argument("--ddp", default="auto", choices=["auto", "p2p", "nvls", "p2p_host", "nccl", "zero"],
@@ -205,7 +209,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), float(d.get("bf16_tflops", 1590.0)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1590.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, 989.0, "data sheet, H100 SXM at 700 W: HBM3 3.35 TB/s, dense FP16 989 TFLOP/s (not reached figures)"
 
 
 # --------------------------------------------------------------------------------------------------
@@ -380,17 +384,18 @@ def run_b200(args):
     from ngp_pl_b200.trainer import Trainer, shard_range
     world, rank, local, pg = dist_setup()
     dev = torch.device("cuda", local)
+    torch.manual_seed(rank)  # every draw outside the trainer's and the bank's own generators: same inputs run to run
     wl = WORKLOADS[args.workload]
     n_rays = wl["n_rays"]
     scene = make_scene(args.workload)
     esf = scene.exp_step_factor
     bank = synth.RayBank(scene, n_images=N_TRAIN_IMAGES, device=dev, seed=rank)  # every rank: own images order/sampling
-    # auto: the peer-load kernel up to 4 GPUs, the NVSwitch-reduced variant beyond (measured ms/step p2p vs nvls: N=2 0.390 vs
-    # 0.425, N=4 0.381 vs 0.387, N=8 0.447 vs 0.431; profiles/r02_bench_n2_*.json, r02_exchange_residency.txt,
-    # r02_bench_n8_*.json); falls back to p2p without a multicast mapping
+    # auto: the peer-load kernel up to 4 GPUs, the NVSwitch-reduced variant beyond; falls back to p2p without a multicast
+    # mapping
     ddp_mode = args.ddp if args.ddp != "auto" else ("p2p" if world <= 4 else "nvls")
     tkw = dict(n_rays=n_rays, lr=1e-2, exp_step_factor=esf, bg=(scene.bg,) * 3, process_group=pg, world_size=world, rank=rank, seed=rank)
     model = NGP(scene.scale).to(dev)
+    mode_used = ddp_mode
     try:
         tr = Trainer(model, ddp=ddp_mode, **tkw)
     except Exception as e:  # symmetric memory / multicast unavailable: fall back and say so in the line
@@ -400,7 +405,7 @@ def run_b200(args):
         ddp_note = "%s (%s unavailable: %s)" % (fallback, ddp_mode, type(e).__name__)
         model = NGP(scene.scale).to(dev)
         tr = Trainer(model, ddp=fallback, **tkw)
-        ddp_mode = ddp_note
+        ddp_mode, mode_used = ddp_note, fallback
     tr.attach_bank(bank)
     xchk = exchange_check(tr, world, rank) if world > 1 else None
     pretrain = args.pretrain if args.pretrain is not None else 1000
@@ -436,6 +441,19 @@ def run_b200(args):
     tr.check_exchange()
     stats = tr.stats()
     value = world * n_rays * K / (ms * 1e-3)
+    if args.dump_outputs:
+        # The timed step (same captured graphs) on inputs that are the same every run: seeded initial weights, occupancy
+        # and optimiser state, the trainer's first batch. The state the timed steps start from is not: it comes out of
+        # 1,000+ steps whose gradients are fp32 sums accumulated by atomics in arbitrary order, and Adam (eps 1e-15) turns
+        # the sign of a near-zero sum into a full learning-rate step, so two runs' trajectories part.
+        fixed = Trainer(NGP(scene.scale).to(dev), ddp=mode_used, **tkw)
+        fixed.attach_bank(bank)
+        fixed.capture(sample=True)
+        grad = {}
+        fixed.train_step(after_backward=lambda t: grad.update(g=t.G.detach().cpu()))
+        if rank == 0:
+            dump_outputs(args.dump_outputs, fixed, grad["g"])
+        del fixed
 
     # ---- e2e: host batches, H2D every step, loss read back (and waited for) every step ------------------
     n_host = 32
@@ -510,15 +528,7 @@ def run_b200(args):
         # kernel runs right after its producer); cold = after a 256 MB L2 flush
         t = {k: {"warm": timed(f, False), "cold": timed(f, True)} for k, f in (("mlp", f_mlp), ("sc", f_sc), ("fwd", f_fwd))}
         G.zero_()
-        traffic, traffic_src = {}, None
-        prof = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(prof):
-            try:
-                traffic = json.load(open(prof))
-                traffic_src = "profiles/ncu_traffic.json (%s): ncu --set full capture of a c2 step, NOT measured in this run" % \
-                    traffic.get("_source", "capture")
-            except Exception:
-                traffic = {}
+        traffic, traffic_src = {}, None  # no DRAM-traffic capture ships with the project
 
         def entry(kernel, bound, tt, n_, per_sample, peak, unit, note):
             alg = n_ * per_sample
@@ -533,16 +543,15 @@ def run_b200(args):
               entry("k_grid_scatter_merged", "hbm", t["sc"], n_bwd, 1024.0, hbm, "GB/s",
                     "1,024 B/sample gradient RMW, composited samples only"),
               entry("k_ngp_bwd3", "tensor", t["mlp"], n_bwd, 40960.0, tf, "TFLOP/s",
-                    "40,960 FLOP/sample dgrad (mma.sync) + wgrad (tcgen05.mma, TMEM accumulators), composited samples only")]
+                    "40,960 FLOP/sample dgrad (mma.sync) + wgrad (wgmma, register accumulators), composited samples only")]
         roof = dict(max(ks, key=lambda e: e["ms_per_launch"]))  # the dominant kernel of the step
         roof["peak_source"] = which
         roof["traffic_source"] = traffic_src
         roof["kernels"] = ks
         roof["timing"] = "CUDA events around single launches on the current stream, mean of 10 after 3 warm-ups; ms_per_launch = warm L2 " \
                          "(in-step state), ms_per_launch_cold_l2 = after a 256 MB flush"
-        roof["note"] = ("hash table (22.9 MB fp16) and its fp32 gradient (45.8 MB) are L2-resident on B200, so DRAM traffic stays far "
-                        "below the algorithmic bytes; the physical limiters are L1 wavefronts of divergent 4-B gathers / 8-B reductions "
-                        "and, for the MLP backward, the latency of its per-row dgrad chain (profiles/)")
+        roof["note"] = ("hash table (22.9 MB fp16) and its fp32 gradient (45.8 MB) are gathered / reduced at random: much of it is "
+                        "served by the 50 MB L2, so DRAM traffic differs from the algorithmic bytes")
 
     # ---- 800x800 render FPS with the trained model (BASELINE config 3), views sharded over the ranks ------------
     fps = None
@@ -583,7 +592,7 @@ def run_b200(args):
                         "zero": "NCCL reduce_scatter + sharded Adam + all_gather(fp16 params)",
                         "nccl": "NCCL all_reduce + full Adam"}.get(ddp_mode, ddp_mode))),
                    "pretrain_steps": pretrain,
-                   "l2": "no explicit flush: each step streams params+grads+Adam moments (~230 MB) > 126 MB L2",
+                   "l2": "no explicit flush: each step streams params+grads+Adam moments (~230 MB) > 50 MB L2",
                    "samples_per_ray_marched": stats["rm_samples"] / n_rays, "samples_per_ray_composited": stats["vr_samples"] / n_rays,
                    "samples_per_ray_in_backward": stats["bw_samples"] / n_rays,
                    "train_psnr_last_batch": stats["psnr"]},
@@ -604,6 +613,18 @@ def run_b200(args):
         except Exception as e:  # the oracle is only a reported baseline; never let it sink the bench line
             line["cpu_baseline"] = {"unavailable": repr(e)}
     print(json.dumps(line))
+
+
+def dump_outputs(out_dir, tr, grad):
+    """A step's per-ray render of the batch (rgb, opacity, depth), its loss terms (Trainer.scalars[1:4]: loss scale, sum of
+    squared errors, sum of opacity entropies) and its whole gradient before Adam (flat, Trainer.P layout: 45.8 MB for c2).
+    The parameters after Adam are left out: eps 1e-15 makes the update of a gradient at rounding level arbitrary."""
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    out = {"rgb": tr.rgb, "opacity": tr.opacity, "depth": tr.depth, "loss_terms": tr.scalars[1:4], "grad": grad}
+    for k, v in out.items():
+        np.save(os.path.join(out_dir, k + ".npy"), np.ascontiguousarray(v.detach().float().cpu().numpy(), np.float32))
 
 
 def render_fps(render_fn, scene, dev, n_views, world=1, rank=0):
@@ -728,7 +749,7 @@ def run_reference(args):
         "clocks": clocks,
         "cpu_baseline": {"value": value, "unit": "rays/s", "cores": 0, "kind": "reference",
                          "sample": "the reference has NO CPU path (every op TORCH_CHECKs is_cuda); this is its own GPU path on the "
-                                   "same B200, all %d steps of the workload" % K},
+                                   "same GPU, all %d steps of the workload" % K},
         "e2e": {"value": value, "unit": "rays/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
     if not args.no_fps:

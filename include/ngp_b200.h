@@ -1,4 +1,4 @@
-/* ngp_b200.h -- C ABI of the B200-native (sm_100a) hot path of kwea123/ngp_pl.
+/* ngp_b200.h -- C ABI of the H100-native (sm_90a) hot path of kwea123/ngp_pl.
  *
  * This is the drop-in boundary. The reference's native surface for this path is the pybind11 module
  * `vren` (reference models/csrc/binding.cpp:234-250, prototypes in models/csrc/include/utils.h:9-126)
@@ -406,7 +406,7 @@ int ngp_render_infer(const NgpNet* net, const NgpInferCfg* cfg, const float* ray
  * condition a kernel sets from the alive count): init -> while (rays alive and samples < sample_budget) { round } ->
  * finish. One graph launch per call, no host read-back at all (the reference's loop synchronises >= 3 times per round,
  * rendering.py:75-105). The instantiated graph is cached per (device, every pointer argument, *net, *cfg) -- up to 8
- * entries, rebuilt on a miss (~1 ms) -- so callers should render from the same buffers frame after frame. Not thread-safe.
+ * entries, rebuilt on a miss -- so callers should render from the same buffers frame after frame. Not thread-safe.
  * Returns a cudaError_t if the driver cannot build conditional graph nodes (callers may then fall back to
  * ngp_render_infer). */
 int ngp_render_infer_frame(const NgpNet* net, const NgpInferCfg* cfg, const float* rays_o, const float* rays_d,

@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) hot path of Instant-NGP behind the operator surface of kwea123/ngp_pl.
+"""H100-native (sm_90a) hot path of Instant-NGP behind the operator surface of kwea123/ngp_pl.
 
     ngp_pl_b200.vren               drop-in for the reference's pybind11 module `vren` (12 operators)
     ngp_pl_b200.tcnn               tinycudann-shaped modules (NetworkWithInputEncoding, Encoding, Network)

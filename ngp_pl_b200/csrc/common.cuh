@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of the ngp_pl hot path.
+// Shared helpers for the sm_90a kernels of the ngp_pl hot path.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -49,13 +49,13 @@ __device__ __forceinline__ void trace_mark(unsigned long long* buf, int id) {  /
 
 static inline int ngp_div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-// Number of SMs of the current device (148 on B200); cached per process.
+// Number of SMs of the current device (132 on H100 SXM); cached per process.
 static inline int ngp_sm_count() {
     static int sms = 0;
     if (sms == 0) {
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
     }
     return sms;
 }
@@ -88,7 +88,7 @@ __device__ __forceinline__ float warp_scan_mul(float v, int lane) {
     return v;
 }
 
-// L2 eviction-priority hints. The optimiser streams ~400 MB (params, moments, gradients) through the 126 MB L2 once per
+// L2 eviction-priority hints. The optimiser streams ~400 MB (params, moments, gradients) through the 50 MB L2 once per
 // step; without hints that evicts the fp16 hash table (24 MB), the zeroed gradient table (49 MB) and the occupancy
 // bitfield which the next step's kernels gather from / reduce into, and those kernels then run from DRAM.
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {

@@ -118,9 +118,8 @@ __device__ __forceinline__ float2 grid_lookup(const uint32_t* __restrict__ table
 // The two x-corners of a cell (k, k+1) sit in ONE aligned entry pair whenever their indices differ only in bit 0: for a
 // hashed level whenever gx is even ((x ^ t) and ((x+1) ^ t)), for a dense level whenever the first index is even (and the
 // pair does not straddle the wrap). The scatter uses that: one 16-byte red.global.add.v4.f32 instead of two 8-byte ones
-// (one L2 atomic transaction; measured -1.5 % on the kernel warm, -5 % cold). The same trick in the GATHER (aligned 8-byte
-// pair load + predicated load of the unpaired corner) and a software-pipelined gather were measured SLOWER than the plain
-// eight 4-byte loads (80.6 / 79.7 vs 77.6 us; profiles/r02_variant_sweep.txt) and are not kept.
+// (one L2 atomic transaction). The same trick in the GATHER (aligned 8-byte pair load + predicated load of the unpaired
+// corner) and a software-pipelined gather were slower than the plain eight 4-byte loads and are not kept.
 // the 8 corner contributions acc[2k], acc[2k+1] of one cell into the gradient table of a level, x-pairs merged when aligned
 __device__ __forceinline__ void grid_scatter_cell_paired(const float* lvl /* level base, float2 per entry */, const uint32_t (&idx)[8],
                                                          const float (&acc)[16]) {

@@ -1,4 +1,4 @@
-// Sync-free inference render for sm_100a: what render(test_time=True) does (reference
+// Sync-free inference render for sm_90a: what render(test_time=True) does (reference
 // models/rendering.py:46-118) as a device-side wavefront.
 //
 // The reference loops on the host: march N more samples for every alive ray, evaluate the network,
@@ -29,9 +29,8 @@
 //   N_samples >= INFER_STAGE (few rays, many samples each) -> one WARP per ray (march_ray_warp: 32 chain points probed side
 //       by side), samples written straight to the ray's own N_samples slots, unused slots marked ray_idx = -1 (the network
 //       kernel skips their gathers).
-//   Measured per round at ~500 k samples (profiles/r02_infer_launches_*.md): thread-per-ray 110-146 us with the generic
-//   visit, warp-per-ray 143-208 us when applied to rounds of 2-7 samples per ray -- so the warp regime is kept for the late
-//   rounds only, and the thread-per-ray visit is specialised (no frexp/scalbn/division with one cascade, constant step).
+//   On rounds of 2-7 samples per ray the warp regime is slower than thread-per-ray, so it is kept for the late rounds
+//   only, and the thread-per-ray visit is specialised (no frexp/scalbn/division with one cascade, constant step).
 // state: [0] N_samples of this round (0 = loop over)  [1] `samples` so far  [2] slots the network evaluates this round
 //        [3] rounds run  [4] samples marched this round  [5] 1 = warp-per-ray regime  [6] finished-block ticket
 #define INFER_STAGE 8  // thread-per-ray regime below this many samples per ray and round (= its staging slots per thread)

@@ -1,4 +1,4 @@
-// Fused NGP network kernels for sm_100a: hash-grid gather + trilinear interpolation + density MLP +
+// Fused NGP network kernels for sm_90a: hash-grid gather + trilinear interpolation + density MLP +
 // exp + SH-4 + rgb MLP + sigmoid in ONE forward kernel, and ONE backward kernel that recomputes the
 // activations, runs dgrad/wgrad on the tensor cores and scatters hash-table gradients with 8-byte
 // vector reductions. Replaces the three tinycudann modules of reference models/networks.py:36-77 and
@@ -6,7 +6,7 @@
 #include "common.cuh"
 #include "hashgrid.cuh"
 #include "mlp.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 #include "../../include/ngp_b200.h"
 #include <math.h>
 #include <stdlib.h>
@@ -990,24 +990,24 @@ k_ngp_bwd2(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
 }
 
 // -------------------------------------------------------------------------------------------------
-// backward, tcgen05 variant (default): the dgrad chain stays on mma.sync fragments in sixteen ROW warps, but the five
-// WEIGHT-GRADIENT GEMMs (dW = dOut^T * In over the 256 staged rows of a block: K = 256, M, N <= 64) are issued by a
-// seventeenth ISSUER warp as tcgen05.mma with both operands read from shared memory through matrix descriptors and the fp32
-// accumulators in TMEM (160 columns, alive for the CTA's whole lifetime; k_ngp_bwd2 keeps 20 accumulator registers per
-// thread and spends 1,280 mma.sync + 2,560 ldmatrix per block on them). The activations are staged in the canonical
-// MN-major no-swizzle layout (umma.cuh); the out-gradient of a layer goes to one of two buffers, so the tensor core can
-// still be reading layer L's while the warps stage layer L+1's.
+// backward, warpgroup-MMA variant (default): the dgrad chain stays on mma.sync fragments in twelve ROW warps, but the five
+// WEIGHT-GRADIENT GEMMs (dW = dOut^T * In over the 192 staged rows of a block: K = 192, M = 64, N <= 64) are issued by a
+// dedicated MMA WARPGROUP (warps 12-15) as wgmma.mma_async with both operands read from shared memory through matrix
+// descriptors and the fp32 accumulators in that warpgroup's registers (64 x 160, 80 a thread, alive for the CTA's whole
+// lifetime; k_ngp_bwd2 keeps 20 accumulator registers per row thread and spends 1,280 mma.sync + 2,560 ldmatrix per block on
+// them). The activations are staged in the canonical MN-major no-swizzle layout (wgmma.cuh); the out-gradient of a layer
+// goes to one of two buffers, so the tensor core can still be reading layer L's while the warps stage layer L+1's.
 // Synchronisation is by mbarriers, not CTA barriers: a row thread that has staged its rows of a layer ARRIVES on that
-// layer's `staged` barrier and carries on with its dgrad; the issuer WAITS on it, issues the 16 MMAs of the layer's GEMM and
-// commits them to the `done` barrier of the buffer they read, which row threads wait on only before they overwrite that
-// buffer two layers later. One CTA barrier per 256-row block is left (ticket broadcast + reuse of the activation tiles);
-// k_ngp_bwd2 has eleven. TMEM columns: [0,16) W3r^T  [16,80) W2r  [80,112) W1r  [112,128) W2d^T  [128,160) W1d.
+// layer's `staged` barrier and carries on with its dgrad; the MMA warpgroup WAITS on it, issues the 12 wgmma of the layer's
+// GEMM, waits for them and arrives on the `done` barrier of the buffer they read, which row threads wait on only before they
+// overwrite that buffer two layers later. One CTA barrier per 192-row block is left (ticket broadcast + reuse of the
+// activation tiles); k_ngp_bwd2 has eleven. Twelve row warps: a 512-thread block keeps the 128 registers a thread the row
+// path needs without spilling (sixteen would leave 96).
 // -------------------------------------------------------------------------------------------------
-#define B3_WARPS 16
+#define B3_WARPS 12
 #define B3_ROW_THREADS (B3_WARPS * 32)
-#define B3_THREADS (B3_ROW_THREADS + 32)
+#define B3_THREADS (B3_ROW_THREADS + 128)
 #define B3_ROWS (B3_WARPS * 16)
-#define B3_TMEM_COLS 256
 struct Bwd3Smem {
     MlpWeightsFwd wf;
     __align__(128) __half feat[B3_ROWS * 32];
@@ -1016,9 +1016,8 @@ struct Bwd3Smem {
     __align__(128) __half r1[B3_ROWS * 64];
     __align__(128) __half r2[B3_ROWS * 64];
     __align__(128) __half dbuf[2][B3_ROWS * 64];  // out-gradient of the layer being processed, alternating
-    __align__(8) uint64_t done[2];                // completion of the MMAs that read dbuf[b]
+    __align__(8) uint64_t done[2];                // completion of the MMAs that read dbuf[b] (one arrival per MMA warp)
     uint64_t staged[5];                           // all rows of layer L are staged (one arrival per row warp and block)
-    uint32_t tmem_base;
     int blk[2];
 };
 
@@ -1047,22 +1046,42 @@ __device__ __forceinline__ void load_canon(const __half* __restrict__ src, int C
         A[0][kt][3] = *reinterpret_cast<const uint32_t*>(b1 + (2 * kt + 1) * 64);
     }
 }
-// D[M=64][N] (+)= A^T B over the B3_ROWS staged rows: A = tile of CA channels (its first 64 are M), B = tile of CB channels
-// (its first N are N); one elected thread
-__device__ __forceinline__ void umma_wgrad(uint32_t tmem_d, const __half* A, int CA, const __half* B, int CB, int N, bool first) {
-    const uint32_t idesc = umma_instr_desc_f16(64, N);
-    const uint32_t lbo_a = (uint32_t)CA * 16u, lbo_b = (uint32_t)CB * 16u;  // bytes between 8-row blocks: C/8 * 128
-    uint64_t ad = umma_smem_desc(A, lbo_a, 128), bd = umma_smem_desc(B, lbo_b, 128);
+// D[64][N] += A^T B over the B3_ROWS staged rows: A = tile of 64 channels (M), B = tile of N channels; the whole MMA
+// warpgroup executes it and returns when the MMAs have completed (their operands may then be overwritten)
+template <int N>
+__device__ __forceinline__ void wgmma_wgrad(float (&d)[N / 2], const __half* A, const __half* B) {
+    const uint32_t lbo_a = 64u * 16u, lbo_b = (uint32_t)N * 16u;  // bytes between 8-row blocks: C/8 * 128
+    uint64_t ad = wgmma_smem_desc(A, lbo_a, 128), bd = wgmma_smem_desc(B, lbo_b, 128);
     const uint64_t a_step = (uint64_t)((2u * lbo_a) >> 4), b_step = (uint64_t)((2u * lbo_b) >> 4);  // 16 rows, in 16-byte units
-#pragma unroll 4
+    wgmma_fence_operand(d);
+    wgmma_fence();
+#pragma unroll
     for (int ks = 0; ks < B3_ROWS / 16; ++ks) {
-        umma_mma_f16(tmem_d, ad, bd, idesc, (first && ks == 0) ? 0u : 1u);
+        wgmma_f16<N>(d, ad, bd);
         ad += a_step;  // the start-address field is the low 14 bits; the tiles end below 256 KB, so no carry leaves it
         bd += b_step;
     }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(d);
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* mbar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"((uint32_t)__cvta_generic_to_shared(mbar)) : "memory");
+// this thread's fragment of a D[64][N] accumulator (rows m0, m0 + 8; columns 8 j + 2 q, + 1) * inv_scale -> dW by fp32
+// reductions: dW[m][n] (row-major, ld) or, TRANSPOSED, dW[n][m]
+template <int N, bool TRANSPOSED>
+__device__ __forceinline__ void wgmma_acc_flush(const float (&d)[N / 2], float* dW, int ld, int m0, int q, float inv_scale) {
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int m = m0 + 8 * h, c = 8 * j + 2 * q;
+            const float v0 = d[4 * j + 2 * h] * inv_scale, v1 = d[4 * j + 2 * h + 1] * inv_scale;
+            if (TRANSPOSED) {
+                asm volatile("red.global.add.f32 [%0], %1;" ::"l"(dW + c * ld + m), "f"(v0) : "memory");
+                asm volatile("red.global.add.f32 [%0], %1;" ::"l"(dW + (c + 1) * ld + m), "f"(v1) : "memory");
+            } else {
+                red_add_f32x2(dW + m * ld + c, v0, v1);
+            }
+        }
 }
 
 __global__ void __launch_bounds__(B3_THREADS, 1)
@@ -1076,7 +1095,7 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
     load_weights_fwd(S.wf, wd, wr, threadIdx.x, B3_THREADS);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
-    const bool issuer = warp == B3_WARPS;
+    const bool mma_wg = warp >= B3_WARPS;
     const int64_t n = bwd_count(smp);
     const int32_t* __restrict__ live = smp.live_idx;
     const int64_t n_mtiles = (n + 15) / 16;
@@ -1085,21 +1104,61 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
     const float inv_scale = 1.0f / scale;
     const int row0 = 16 * warp;
 
-    if (warp == 0) tmem_alloc<B3_TMEM_COLS>(&S.tmem_base);
     if (threadIdx.x == 0) {
-        mbar_init(&S.done[0], 1);
-        mbar_init(&S.done[1], 1);
+        mbar_init(&S.done[0], 4);
+        mbar_init(&S.done[1], 4);
 #pragma unroll
         for (int l = 0; l < 5; ++l) mbar_init(&S.staged[l], B3_WARPS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         S.blk[0] = sched ? atomicAdd(&sched[0], 1) : (int)blockIdx.x;
     }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem = S.tmem_base;
-    uint32_t commits[2] = {0u, 0u};  // MMA batches committed to done[b] so far (every thread counts the same)
-    int n_done = 0;                  // blocks processed by this CTA
+    uint32_t commits[2] = {0u, 0u};  // MMA batches signalled on done[b] so far (every thread counts the same)
+
+    if (mma_wg) {
+        // ================= MMA warpgroup: one GEMM per layer, as soon as the layer's rows are staged =================
+        // accumulators: W3r^T [in 64][out 16], W2r [64][64], W1r [64][32], W2d^T [in 64][out 16], W1d [64][32]
+        float a3r[8], a2r[32], a1r[16], a2d[8], a1d[16];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) a3r[i] = a2d[i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) a1r[i] = a1d[i] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) a2r[i] = 0.f;
+        auto signal = [&](int b) {  // the GEMM that read dbuf[b] has completed
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&S.done[b]);
+        };
+        int n_done = 0;  // blocks processed by this CTA
+        for (int it = 0;; ++it) {
+            const int64_t blk = S.blk[it & 1];
+            if (blk >= n_blks) break;
+            ++n_done;
+            __syncthreads();  // (the block's CTA barrier: see the row warps)
+            const uint32_t par = (uint32_t)it & 1u;
+            mbar_wait(&S.staged[0], par);
+            wgmma_wgrad<16>(a3r, S.r2, S.dbuf[0]);   signal(0);
+            mbar_wait(&S.staged[1], par);
+            wgmma_wgrad<64>(a2r, S.dbuf[1], S.r1);   signal(1);
+            mbar_wait(&S.staged[2], par);
+            wgmma_wgrad<32>(a1r, S.dbuf[0], S.rin);  signal(0);
+            mbar_wait(&S.staged[3], par);
+            wgmma_wgrad<16>(a2d, S.hid, S.dbuf[1]);  signal(1);
+            mbar_wait(&S.staged[4], par);
+            wgmma_wgrad<32>(a1d, S.dbuf[0], S.feat); signal(0);
+        }
+        sched_finish(sched);
+        // ---- flush the weight gradients: registers -> fp32 reductions ----
+        if (n_done > 0) {
+            const int m0 = 16 * (warp - B3_WARPS) + g;
+            wgmma_acc_flush<16, true>(a3r, grad_rgb + 2048 + 4096, 64, m0, q, inv_scale);  // W3r (16 x 64), accumulated transposed
+            wgmma_acc_flush<64, false>(a2r, grad_rgb + 2048, 64, m0, q, inv_scale);        // W2r (64 x 64)
+            wgmma_acc_flush<32, false>(a1r, grad_rgb, 32, m0, q, inv_scale);               // W1r (64 x 32)
+            wgmma_acc_flush<16, true>(a2d, grad_enc + 2048, 64, m0, q, inv_scale);         // W2d (16 x 64), transposed
+            wgmma_acc_flush<32, false>(a1d, grad_enc, 32, m0, q, inv_scale);               // W1d (64 x 32)
+        }
+        return;
+    }
 
     // ---- software-pipelined row fetch (row warps): state of the NEXT block's two rows of this lane ----
     bool pre_valid[2] = {false, false};
@@ -1151,10 +1210,8 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
         }
         (void)nblk;
     };
-    if (!issuer) {
-        fetch_hop1(S.blk[0]);
-        fetch_hop2(S.blk[0]);
-    }
+    fetch_hop1(S.blk[0]);
+    fetch_hop2(S.blk[0]);
 
     // wait until the most recent MMA batch that read dbuf[b] (and everything issued before it) has completed
     auto wait_buf = [&](int b) {
@@ -1165,30 +1222,6 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
         const int64_t blk = S.blk[it & 1];
         if (blk >= n_blks) break;
         if (threadIdx.x == 0) S.blk[(it + 1) & 1] = sched ? atomicAdd(&sched[0], 1) : (int)(blk + gridDim.x);
-        ++n_done;
-
-        if (issuer) {
-            // ================= issuer warp: one GEMM per layer, as soon as the layer's rows are staged =================
-            __syncthreads();  // (the block's CTA barrier: see the row warps)
-            const uint32_t par = (uint32_t)it & 1u;
-            const bool first = it == 0;
-            if (lane == 0) {
-                mbar_wait(&S.staged[0], par); tcgen05_fence_after();
-                umma_wgrad(tmem + 0u, S.r2, 64, S.dbuf[0], 16, 16, first);   umma_commit(&S.done[0]);
-                mbar_wait(&S.staged[1], par); tcgen05_fence_after();
-                umma_wgrad(tmem + 16u, S.dbuf[1], 64, S.r1, 64, 64, first);  umma_commit(&S.done[1]);
-                mbar_wait(&S.staged[2], par); tcgen05_fence_after();
-                umma_wgrad(tmem + 80u, S.dbuf[0], 64, S.rin, 32, 32, first); umma_commit(&S.done[0]);
-                mbar_wait(&S.staged[3], par); tcgen05_fence_after();
-                umma_wgrad(tmem + 112u, S.hid, 64, S.dbuf[1], 16, 16, first); umma_commit(&S.done[1]);
-                mbar_wait(&S.staged[4], par); tcgen05_fence_after();
-                umma_wgrad(tmem + 128u, S.dbuf[0], 64, S.feat, 32, 32, first); umma_commit(&S.done[0]);
-            }
-            __syncwarp();
-            commits[0] += 3u;
-            commits[1] += 2u;
-            continue;
-        }
 
         // ================= row warps =================
         // The rows of THIS block were fetched while the previous block was processed (hop 1: live index, right after that
@@ -1379,44 +1412,7 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
         }
     }
 
-    sched_finish(sched);
-    // ---- flush the weight gradients: TMEM -> registers -> fp32 reductions. Row m of an M = 64 accumulator sits in lane
-    //      (m % 16) + 32 (m / 16): warp w < 4 reads its 32 lanes, threads 0..15 of it hold rows 16 w + t ----
-    wait_buf(0);
-    wait_buf(1);
-    tcgen05_fence_after();
-    if (n_done > 0 && warp < 4) {
-        const int m = 16 * warp + lane;  // (meaningful for lane < 16)
-        const uint32_t lane_base = tmem + ((uint32_t)(32 * warp) << 16);
-        uint32_t r[16];
-        auto flush = [&](uint32_t col, int ncols, float* dW, int ld, bool transposed) {
-            for (int c0 = 0; c0 < ncols; c0 += 16) {
-                tmem_ld_32x32b_x16(lane_base + col + (uint32_t)c0, r);
-                if (lane < 16) {
-                    if (transposed) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            asm volatile("red.global.add.f32 [%0], %1;" ::"l"(dW + (c0 + j) * ld + m),
-                                         "f"(__uint_as_float(r[j]) * inv_scale)
-                                         : "memory");
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 16; j += 4)  // 16 consecutive columns of one row: four 16-byte reductions
-                            red_add_f32x4(dW + m * ld + c0 + j, __uint_as_float(r[j]) * inv_scale, __uint_as_float(r[j + 1]) * inv_scale,
-                                          __uint_as_float(r[j + 2]) * inv_scale, __uint_as_float(r[j + 3]) * inv_scale);
-                    }
-                }
-            }
-        };
-        flush(0u, 16, grad_rgb + 2048 + 4096, 64, true);   // W3r (16 x 64), accumulated transposed
-        flush(16u, 64, grad_rgb + 2048, 64, false);        // W2r (64 x 64)
-        flush(80u, 32, grad_rgb, 32, false);               // W1r (64 x 32)
-        flush(112u, 16, grad_enc + 2048, 64, true);        // W2d (16 x 64), transposed
-        flush(128u, 32, grad_enc, 32, false);              // W1d (64 x 32)
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_free<B3_TMEM_COLS>(tmem);
+    sched_finish(sched);  // (the MMA warpgroup flushes the weight gradients)
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1539,7 +1535,7 @@ extern "C" int ngp_net_backward_mlp(const NgpNet* net, const NgpSamples* smp, co
             if (dev >= 0 && dev < 64) __atomic_store_n(&attr_set[dev], 1, __ATOMIC_RELEASE);
         }
     }
-    static int variant = -1;  // NGP_BWD_VARIANT (env, read once): 2 = tcgen05 weight gradients (default), 1 = k_ngp_bwd2, 0 = k_ngp_bwd
+    static int variant = -1;  // NGP_BWD_VARIANT (env, read once): 2 = wgmma weight gradients (default), 1 = k_ngp_bwd2, 0 = k_ngp_bwd
     if (variant < 0) {
         const char* e = getenv("NGP_BWD_VARIANT");
         variant = e ? atoi(e) : 2;

@@ -1,4 +1,4 @@
-// Fused training path for sm_100a: everything render(test_time=False) does (reference
+// Fused training path for sm_90a: everything render(test_time=False) does (reference
 // models/rendering.py:11-43,:121-163) plus loss, optimiser, batch assembly and the occupancy-grid
 // refresh, as a handful of stream-ordered launches with NO host synchronisation (sample counts never
 // leave the device), so a whole optimiser step can be captured in one CUDA graph.
@@ -10,7 +10,7 @@
 #include <cub/device/device_select.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
 
-static inline int one_thread_per_ray_block(int n_rays) { return n_rays >= 148 * 128 * 4 ? 128 : 32; }
+static inline int one_thread_per_ray_block(int n_rays) { return n_rays >= ngp_sm_count() * 128 * 4 ? 128 : 32; }
 
 // -------------------------------------------------------------------------------------------------
 // 1. AABB + near clamp + jittered march, ONE pass: samples go to a per-ray staging row
@@ -329,7 +329,7 @@ __global__ void __launch_bounds__(CL_WARPS * 32) k_train_composite_loss(const Ng
     // The ray's first CL_CACHE trips of 32 samples are loaded up front (independent loads, one exposed latency instead of
     // one per trip) and kept in registers for the backward sweep; longer rays continue trip by trip from memory. The
     // kernel is two waves of warps and lasts as long as its longest rays: with the generic helpers (a dependent load ->
-    // scan chain per trip, twice) that was 24 us (profiles/r02_step_timeline_n1.txt). Arithmetic and its order are those of
+    // scan chain per trip, twice) those chains were what it waited on. Arithmetic and its order are those of
     // composite_ray_warp / composite_ray_warp_bwd (composite.cuh), minus the depth and ws scans whose gradients are zero.
     CLSample sm[CL_CACHE];
 #pragma unroll
@@ -454,8 +454,7 @@ __global__ void __launch_bounds__(CL_WARPS * 32) k_train_composite_loss(const Ng
         m = warp_max(m);
     }
     // Per-ray sums, the loss-scale maximum and the live-list allocation go through ONE set of atomics per BLOCK (8 rays):
-    // five same-address atomics per ray serialise in the L2 atomic unit -- 41 k of them made this kernel 41 us
-    // (profiles/r02_launches_step_c2.md) although its arithmetic is a few microseconds.
+    // five same-address atomics per ray serialise in the L2 atomic unit.
     __shared__ float s_se[CL_WARPS], s_ent[CL_WARPS], s_m[CL_WARPS];
     __shared__ int s_tot[CL_WARPS], s_comp[CL_WARPS], s_base;
     const int wib = threadIdx.x >> 5;
@@ -516,8 +515,7 @@ extern "C" int ngp_render_train_step(const NgpNet* net, const NgpTrainCfg* cfg, 
     static int cl_cache = -1;
     if (cl_cache < 0) {
         const char* e = getenv("NGP_CL_CACHE");
-        cl_cache = e ? atoi(e) : 4;  // measured in the step on the c2 scene (rays: median 0, p90 138, max 415 samples):
-                                     // 8 -> 20.1 us (80 regs), 4 -> 17.3 us (64 regs), 2 -> 17.7 us
+        cl_cache = e ? atoi(e) : 4;  // 128 samples of a ray in registers (64 regs)
     }
 #define NGP_LAUNCH_CL(C)                                                                                                   \
     k_train_composite_loss<C><<<ngp_div_up(n, CL_WARPS), CL_WARPS * 32, 0, st>>>(                                          \
@@ -695,9 +693,7 @@ extern "C" int ngp_adam_step(float* params, float* grads, float* exp_avg, float*
     cudaStream_t st = (cudaStream_t)stream;
     if (n > 0) {
         // 2 resident blocks per SM (two 64-byte groups per thread in flight) saturate HBM and leave registers for the
-        // next step's march, which a trainer overlaps with this kernel on another stream (measured inside the pipelined
-        // step on B200: 0.378 ms/step with 2 blocks/SM; 3 -> 0.394, 4 -> 0.390, 1 -> 0.411; a shared-memory staged
-        // cp.async variant: 0.393)
+        // next step's march, which a trainer overlaps with this kernel on another stream
         int grid = ngp_div_up((n >> 2) + 1, 256);
         const int cap = ngp_sm_count() * 2;
         if (grid > cap) grid = cap;
@@ -912,8 +908,8 @@ k_adam_fused(const FusedPeers peers, const int world, const int rank, float* __r
     const uint64_t stream_pol = l2_policy_evict_first();
     const bool mc_in = peers.mc_grads != nullptr, mc_out = peers.mc_params_half != nullptr;
     // U float4 groups per thread per trip, their remote loads issued back to back before anything waits on them: one
-    // multimem.ld_reduce (or one round of peer loads) per trip made the loop a chain of ~30 NVLink round trips per thread
-    // and the data phase 95 us at N=4 although it moves 12 MB in and 6 MB out per rank (profiles/r02_step_timeline_n4.txt)
+    // multimem.ld_reduce (or one round of peer loads) per trip would make the loop a chain of ~30 NVLink round trips per
+    // thread
     constexpr int U = W <= 2 ? 4 : (W <= 4 ? 2 : 1);  // peer-load path: U * W float4 in flight per thread
     constexpr int UM = 4;                             // multimem path: the switch reduces, one float4 per group
     const int64_t tid = blockIdx.x * (int64_t)blockDim.x + threadIdx.x, nthr = (int64_t)gridDim.x * blockDim.x;
@@ -1028,9 +1024,8 @@ extern "C" int ngp_adam_step_fused(int world, int rank, const uint64_t* peer_gra
     int grid = ngp_div_up(work > 0 ? work : 1, 256 * 4);
     // Resident blocks per SM. The kernel is NVLink-bound and spends part of its life waiting at its barriers, and while 3
     // blocks per SM are resident (80 registers x 768 threads) no block of the next step's run-ahead march fits beside
-    // them. Measured in the pipelined step (profiles/r02_exchange_residency.txt): N=2 3 -> 0.365, 2 -> 0.388, 1 -> 0.443 ms
-    // (half the table per rank: the kernel's own speed wins); N=4 p2p 3 -> 0.3830, 2 -> 0.3807, 1 -> 0.3831 and nvls
-    // 3 -> 0.398, 2 -> 0.387 (the march's share of the SMs wins). NGP_FUSED_BLOCKS_PER_SM (env, read once) overrides.
+    // them: with two ranks half the table per rank makes the kernel's own speed win (3), beyond that the march's share of
+    // the SMs (2). NGP_FUSED_BLOCKS_PER_SM (env, read once) overrides.
     static int per_sm_env = -1;
     if (per_sm_env < 0) {
         const char* e = getenv("NGP_FUSED_BLOCKS_PER_SM");
@@ -1190,9 +1185,8 @@ __global__ void k_grid_flags(const float* __restrict__ grid, int64_t n, float th
 //   else   : 2*M slots, [0,M) uniform random cells, [M,2M) random occupied cells (key = g3, "none", if there are none)
 // The picked Morton indices are then SORTED (cub radix sort) before the density is evaluated: the result of the refresh does
 // not depend on the order the cells are evaluated in (it is scattered back per cell), but the evaluation does -- 1M cells in
-// random order make every hash-grid gather of a warp hit 32 different sectors and the density pass took 368 us; in Morton
-// order neighbouring threads share cells on the coarse levels, like consecutive samples of a ray do (profiles/
-// r02_step_timeline_n1.txt).
+// random order make every hash-grid gather of a warp hit 32 different sectors; in Morton order neighbouring threads share
+// cells on the coarse levels, like consecutive samples of a ray do.
 __global__ void k_grid_pick_cells(const GridUpd u, int c, const int* __restrict__ occ_list, const int* __restrict__ occ_count,
                                   uint32_t* __restrict__ keys) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1255,40 +1249,62 @@ __global__ void k_grid_scatter(const int* __restrict__ cell_idx, const float* __
     }
 }
 
-// grid = grid < 0 ? grid : max(grid*decay, tmp); accumulate sum / count of the positive cells
+// grid = grid < 0 ? grid : max(grid*decay, tmp); sum / count of the positive cells per block, into part / part_n[block]
 // erode (count_grid != NULL, reference networks.py:258-260): cells seen by few cameras decay faster,
 // decay_i = clamp(decay^(1/count_i), 0.1, 0.95)
 __global__ void k_grid_merge(float* __restrict__ grid, const float* __restrict__ tmp, int64_t n, float decay,
-                             const float* __restrict__ count_grid, float* __restrict__ stats /* [0]=sum, [1]=count */) {
-    float s = 0.f, cnt = 0.f;
+                             const float* __restrict__ count_grid, float* __restrict__ part, unsigned* __restrict__ part_n) {
+    float s = 0.f;
+    unsigned cnt = 0u;
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         float g = grid[i];
         float d = decay;
         if (count_grid) d = fminf(fmaxf(powf(decay, 1.0f / count_grid[i]), 0.1f), 0.95f);
         if (!(g < 0.f)) g = fmaxf(g * d, tmp[i]);
         grid[i] = g;
-        if (g > 0.f) { s += g; cnt += 1.f; }
+        if (g > 0.f) { s += g; cnt += 1u; }
     }
-    // one pair of atomics per BLOCK: ~9.5k warps adding to the same two addresses serialised in L2 and cost more than the
-    // 24 MB this kernel streams
-    __shared__ float sh_s[8], sh_c[8];
+    // per-block partials, summed in a fixed order by k_grid_mean: float atomics would make the mean -- the occupancy
+    // threshold, near which most cells sit right after initialisation -- depend on the order blocks finish in
+    __shared__ float sh_s[8];
+    __shared__ unsigned sh_c[8];
     s = warp_sum(s);
-    cnt = warp_sum(cnt);
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
     if ((threadIdx.x & 31) == 0) {
         sh_s[threadIdx.x >> 5] = s;
         sh_c[threadIdx.x >> 5] = cnt;
     }
     __syncthreads();
     if (threadIdx.x == 0) {
-        float bs = 0.f, bc = 0.f;
+        float bs = 0.f;
+        unsigned bc = 0u;
         for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { bs += sh_s[w]; bc += sh_c[w]; }
-        atomicAdd(&stats[0], bs);
-        atomicAdd(&stats[1], bc);
+        part[blockIdx.x] = bs;
+        part_n[blockIdx.x] = bc;
     }
 }
-__global__ void k_grid_mean(float* __restrict__ stats) {
-    // stats[2] = mean of the positive cells (NaN when there is none, like the reference's empty .mean())
-    stats[2] = stats[0] / stats[1];
+#define MERGE_MAX_BLOCKS 2048
+// one block of 256 threads: stats[0] = sum, [1] = count, [2] = mean of the positive cells (NaN when there is none, like the
+// reference's empty .mean()), every partial added in the same order every time
+__global__ void k_grid_mean(const float* __restrict__ part, const unsigned* __restrict__ part_n, int n_blocks,
+                            float* __restrict__ stats) {
+    __shared__ float sh_s[256];
+    __shared__ unsigned long long sh_c[256];
+    float s = 0.f;
+    unsigned long long c = 0ull;
+    for (int b = threadIdx.x; b < n_blocks; b += 256) { s += part[b]; c += part_n[b]; }
+    sh_s[threadIdx.x] = s;
+    sh_c[threadIdx.x] = c;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if ((int)threadIdx.x < o) { sh_s[threadIdx.x] += sh_s[threadIdx.x + o]; sh_c[threadIdx.x] += sh_c[threadIdx.x + o]; }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        stats[0] = sh_s[0];
+        stats[1] = (float)sh_c[0];
+        stats[2] = sh_s[0] / (float)sh_c[0];
+    }
 }
 
 // workspace layout (all 256-byte aligned), C = cascades:
@@ -1313,6 +1329,7 @@ static size_t cub_temp_bytes(size_t g3) {
 }
 struct GridWs {
     float* tmp; uint8_t* flags; int* occ_list; int* occ_count; int* cell_idx; float* xyz; float* sigma; float* stats;
+    float* part; unsigned* part_n;  // k_grid_merge's per-block partials
     int* tot;  // [0..C]: first slot of each cascade / total; [63]: number of distinct keys of the cascade being picked
     uint32_t* keys; uint32_t* keys_sorted; void* cub_temp; size_t cub_bytes; size_t total;
 };
@@ -1328,6 +1345,8 @@ static GridWs grid_ws(void* workspace, int cascades, size_t g3) {
     g.xyz = (float*)w; w += al256(C * g3 * 12);
     g.sigma = (float*)w; w += al256(C * g3 * 4);
     g.stats = (float*)w; w += 256;
+    g.part = (float*)w; w += al256(MERGE_MAX_BLOCKS * 4);
+    g.part_n = (unsigned*)w; w += al256(MERGE_MAX_BLOCKS * 4);
     g.tot = (int*)w; w += 256;
     g.keys = (uint32_t*)w; w += al256(g3 * 4);
     g.keys_sorted = (uint32_t*)w; w += al256(g3 * 4);
@@ -1413,9 +1432,10 @@ extern "C" int ngp_update_density_grid_eval(const NgpNet* net, float* density_gr
     NGP_TRACE(23, st);
     int grid = ngp_div_up((int64_t)cascades * g3, 256);
     if (grid > ngp_sm_count() * 8) grid = ngp_sm_count() * 8;
-    k_grid_merge<<<grid, 256, 0, st>>>(density_grid, g.tmp, (int64_t)cascades * g3, decay, count_grid, g.stats);
+    if (grid > MERGE_MAX_BLOCKS) grid = MERGE_MAX_BLOCKS;
+    k_grid_merge<<<grid, 256, 0, st>>>(density_grid, g.tmp, (int64_t)cascades * g3, decay, count_grid, g.part, g.part_n);
     NGP_CHECK_LAUNCH();
-    k_grid_mean<<<1, 1, 0, st>>>(g.stats);
+    k_grid_mean<<<1, 256, 0, st>>>(g.part, g.part_n, grid, g.stats);
     NGP_CHECK_LAUNCH();
     NGP_TRACE(24, st);
     // threshold = min(mean, density_threshold) evaluated on the device (fminf ignores a NaN mean)

@@ -1,4 +1,4 @@
-// The twelve `vren` operators of kwea123/ngp_pl re-implemented for sm_100a behind a C ABI.
+// The twelve `vren` operators of kwea123/ngp_pl re-implemented for sm_90a behind a C ABI.
 // Each entry point cites the reference operator it replaces (reference models/csrc/binding.cpp and
 // the kernel behind it). Plain device pointers and sizes only; the caller owns every buffer.
 #include "common.cuh"
@@ -353,7 +353,7 @@ extern "C" size_t ngp_raymarching_train_workspace2(int n_rays, int max_samples) 
 }
 extern "C" size_t ngp_raymarching_train_workspace(int n_rays) { return ngp_raymarching_train_workspace2(n_rays, 0); }
 
-static inline int march_block(int n_rays) { return n_rays >= 148 * 128 * 4 ? 128 : 32; }
+static inline int march_block(int n_rays) { return n_rays >= ngp_sm_count() * 128 * 4 ? 128 : 32; }
 
 extern "C" int ngp_raymarching_train(const float* rays_o, const float* rays_d, const float* hits_t,
                                      const uint8_t* density_bitfield, int cascades, float scale, float exp_step_factor,
@@ -458,7 +458,7 @@ extern "C" int ngp_raymarching_test(const float* rays_o, const float* rays_d, fl
     NGP_CUDA(cudaMemsetAsync(deltas, 0, slots * sizeof(float), (cudaStream_t)stream));
     NGP_CUDA(cudaMemsetAsync(ts, 0, slots * sizeof(float), (cudaStream_t)stream));
     NGP_COUNT_LAUNCHES(4);
-    const int bs = n_alive >= 148 * 128 * 4 ? 128 : 64;
+    const int bs = n_alive >= ngp_sm_count() * 128 * 4 ? 128 : 64;
     k_march_test<<<ngp_div_up(n_alive, bs), bs, 0, (cudaStream_t)stream>>>(
         rays_o, rays_d, hits_t, alive_indices, density_bitfield, cascades, grid_size, scale, exp_step_factor, N_samples,
         max_samples, n_alive, xyzs, dirs, deltas, ts, N_eff_samples);

@@ -1,5 +1,5 @@
 """NGP model with the reference's constructor, attributes, buffers and methods
-(reference models/networks.py:12-269), evaluated by the fused sm_100a kernels in libngp_b200.so.
+(reference models/networks.py:12-269), evaluated by the fused sm_90a kernels in libngp_b200.so.
 
 State-dict keys match the reference: center, xyz_min, xyz_max, half_size, density_bitfield,
 xyz_encoder.params, dir_encoder.params (empty), rgb_net.params (+ density_grid / grid_coords when the

@@ -32,7 +32,7 @@ class _HalfCopy:
     whenever the parameter can have changed behind autograd's back: the modules call `training_forward()` at the top of
     every forward that runs with grad mode on and a parameter that requires grad (an optimiser that writes through `p.data`
     -- apex FusedAdam, the reference's choice at train.py:128-134 -- or an EMA swap does NOT bump `p._version`); otherwise
-    (inference) the copy is refreshed only when (pointer, version) changed. ~25 us for the 11.5 M parameters."""
+    (inference) the copy is refreshed only when (pointer, version) changed."""
 
     def __init__(self):
         self.buf = None

@@ -596,8 +596,6 @@ class Trainer:
         return int(_lib.lib().ngp_launch_count()) + self.graph_launches
 
     def _capture_graph(self, fn):
-        # (capturing the compute / optimiser graphs on a high-priority stream so that their kernels win the block scheduler
-        # over the run-ahead march was measured: no effect on the step, 0.3840 vs 0.3853 ms, profiles/r02_variant_sweep.txt)
         g = torch.cuda.CUDAGraph()
         g.register_generator_state(self.gen)
         n0 = int(_lib.lib().ngp_launch_count())
@@ -673,8 +671,10 @@ class Trainer:
         if self._n_gbuf == 2:
             self._gcur ^= 1
 
-    def train_step(self, sample=True):
-        """one full training step incl. the occupancy refresh cadence of reference train.py:160-163"""
+    def train_step(self, sample=True, after_backward=None):
+        """one full training step incl. the occupancy refresh cadence of reference train.py:160-163. after_backward(self),
+        if given, is called once the step's gradients (self.G) are complete and before the optimiser consumes and
+        clears them"""
         if self.lr_schedule is not None:
             lr = self.lr_schedule.lr_at_step(self.host_step)
             if lr != self.lr:
@@ -685,7 +685,11 @@ class Trainer:
                 torch.cuda.current_stream(self.dev).wait_stream(self._side)  # a staged copy may still be in flight
             self.update_density_grid(warmup=self.host_step < self.warmup_steps)
         if not (self.graph and self._graph_samples == sample):
-            self._step_body(sample)
+            self._prepare(sample)
+            self._compute()
+            if after_backward is not None:
+                after_backward(self)
+            self._update()
             self._premarched = False
             self.host_step += 1
             return
@@ -697,6 +701,8 @@ class Trainer:
             if refresh:  # staged ahead of a refresh: march now, against the refreshed grid (the reference's ordering)
                 self._replay(self.g_prepare[self._cur])
             self._replay(self.g_compute[self._cur][self._gcur])
+            if after_backward is not None:
+                after_backward(self)
             if self._ev_set[self._cur] is None:
                 self._ev_set[self._cur] = torch.cuda.Event()
             self._ev_set[self._cur].record(main)
@@ -721,6 +727,8 @@ class Trainer:
             with torch.cuda.stream(self._side):
                 self._replay(self.g_prepare[1 - self._cur])
         self._replay(self.g_compute[self._cur][self._gcur])
+        if after_backward is not None:
+            after_backward(self)
         self._ev_compute.record(main)
         self._graph_update()
         if ahead:

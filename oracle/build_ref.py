@@ -5,7 +5,7 @@ What this produces (all git-ignored, all under oracle/_ref/, nothing else is wri
   oracle/_ref/vren*.so        the reference's own CUDA extension `vren`, compiled from the sources
                               where they lie under /root/reference/models/csrc (binding.cpp,
                               raymarching.cu, volumerendering.cu, intersection.cu, losses.cu), for
-                              sm_100 with the reference's own flags (-O2, models/csrc/setup.py:26-27).
+                              sm_90 with the reference's own flags (-O2, models/csrc/setup.py:26-27).
   oracle/_ref/ngp_pl/         an *install* of the reference's Python hot-path modules
                               (models/{__init__,custom_functions,networks,rendering}.py, losses.py,
                               metrics.py), byte-identical, so `bench.py --impl reference` and the parity
@@ -90,7 +90,7 @@ def build_vren(verbose=False):
             obj = src + ".o"
             if f.endswith(".cu"):
                 cmd = ["nvcc", "-c", src, "-o", obj, "-O2", "-std=c++17",
-                       "-gencode", "arch=compute_100,code=sm_100",
+                       "-gencode", "arch=compute_90,code=sm_90",
                        "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-w",
                        # the flags torch.utils.cpp_extension always adds for CUDAExtension
                        "-D__CUDA_NO_HALF_OPERATORS__", "-D__CUDA_NO_HALF_CONVERSIONS__",

@@ -1,7 +1,7 @@
 """Performance-grade stand-in for `tinycudann` -- TEST / BASELINE INFRASTRUCTURE ONLY (never imported by ngp_pl_b200/).
 
 `oracle/tcnn_standin.py` is the CHECKER: a per-level / per-corner Python loop with double-precision positions, int64
-modulo and fp32 `F.linear`, written to be read against tinycudann's published algorithm, and ~50 ms per 8192-ray step.
+modulo and fp32 `F.linear`, written to be read against tinycudann's published algorithm, and slow.
 Timing the reference arm with it under-states what the reference's csrc + tinycudann path does, so `bench.py --impl
 reference` runs THIS module instead: the same three classes, the same parameter layout, seeds and fp16 rounding points,
 written the way one writes fast eager PyTorch on a GPU:
@@ -29,8 +29,7 @@ _BUCKET = 32768
 def _pad_rows(x):
     """Pad the batch to a multiple of 32768 rows (tinycudann pads to its batch granularity too). The sample count of a
     training step changes every step; without the padding every GEMM sees a new M and cuBLAS(Lt) re-runs its algorithm
-    heuristics on the host for ~2 ms per call (torch.profiler: aten::mm 1.8 ms of CPU each, 27 ms per step against 8.6 ms of
-    GPU work), which made the arm host-bound."""
+    heuristics on the host on every call, which made the arm host-bound."""
     n = x.shape[0]
     nb = (n + _BUCKET - 1) // _BUCKET * _BUCKET
     return x if nb == n else torch.nn.functional.pad(x, (0, 0, 0, nb - n))

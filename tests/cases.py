@@ -1,4 +1,4 @@
-"""Deterministic parity cases shared by tests/golden/make_golden.py (runs the REAL reference on a B200),
+"""Deterministic parity cases shared by tests/golden/make_golden.py (runs the REAL reference on a GPU),
 the CPU-oracle tests and the GPU parity tests. numpy RandomState only, so every host builds the
 same inputs."""
 import numpy as np
@@ -94,5 +94,43 @@ def composite_case(seed=3, n_rays=96, max_n=300):
     return dict(sigmas=sig, rgbs=rgbs, deltas=deltas, ts=ts, rays_a=rays_a, T_thr=np.float32(1e-4), **g)
 
 
+def composite_test_case():
+    """one round of the test-time compositor: 150 of 200 rays alive, up to 8 samples each, running ray state"""
+    rng = np.random.RandomState(4)
+    n_rays, n_alive, ns = 200, 150, 8
+    alive = rng.permutation(n_rays)[:n_alive].astype(np.int64)
+    sig = np.exp(rng.normal(0, 2.5, (n_alive, ns))).astype(np.float32)
+    rgbs = rng.rand(n_alive, ns, 3).astype(np.float32)
+    dl = np.full((n_alive, ns), 0.01, np.float32)
+    ts = np.cumsum(dl, 1).astype(np.float32)
+    neff = rng.randint(0, ns + 1, n_alive).astype(np.int32)
+    op0 = (rng.rand(n_rays) * 0.9).astype(np.float32)
+    dp0 = rng.rand(n_rays).astype(np.float32)
+    rgb0 = rng.rand(n_rays, 3).astype(np.float32)
+    return dict(alive=alive, sigmas=sig, rgbs=rgbs, deltas=dl, ts=ts, neff=neff, op0=op0, dp0=dp0, rgb0=rgb0)
+
+
 def hits_for(case, oracle):
     return oracle.ray_aabb(case["o"], case["d"], np.zeros(3, np.float32), np.full(3, case["scale"], np.float32), NEAR)
+
+
+# ---- golden fixtures of large outputs (tests/golden/make_golden_render.py and the GPU tests that read them) ----------
+SAMPLE_SEED = 1234
+
+
+def sample_idx(n, k):
+    """a fixed, seeded, sorted sample of k of the indices 0..n-1 (all of them when n <= k)"""
+    if n <= k:
+        return np.arange(n)
+    return np.sort(np.random.RandomState(SAMPLE_SEED).choice(n, k, replace=False))
+
+
+def digest(a):
+    """SHA-256 of an array's bytes (C order), as 32 uint8: stands in for a whole array that a test checks bit for bit"""
+    import hashlib
+    return np.frombuffer(hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest(), np.uint8)
+
+
+def target_rgb(n, seed):
+    """seeded target colours for the loss of a parity render"""
+    return np.random.RandomState(seed).rand(n, 3).astype(np.float32)

@@ -2,7 +2,7 @@
 
 ngp_trace_set() makes the step's entry points enqueue a one-thread kernel after each of their kernels that appends
 {id, %globaltimer}; the stamps are captured into the CUDA graphs, so the timeline is the graph-replayed, two-stream
-steady state. Each stamp costs ~2 us of launch chain, so the traced step is ~10 % slower than the untraced one (both are
+steady state. Each stamp adds to the launch chain, so the traced step is slower than the untraced one (both are
 printed); read it for WHERE time goes, not for absolute numbers.
 
     python tools/step_timeline.py [steps] [n_steps_to_print] [ddp mode]
