@@ -437,7 +437,8 @@ def test_stage_batch_prefetch_matches_set_batch():
         tr.set_batch(*host[0])
         tr.capture(sample=False)
         # no occupancy refresh inside the comparison: right after initialisation all cell densities sit on the mean that
-        # thresholds them, so the refreshed bitfield depends on the rounding of a float-atomic sum
+        # thresholds them, so the refreshed bitfield would turn on the last bits of the weights, which the two runs'
+        # gradient atomics already let drift apart
         tr.host_step = 1
         log = []
         if prefetch:

@@ -258,7 +258,6 @@ def test_refresh_picked_ahead_equals_refresh_in_line(which):
         out.append(grids)
     for (ga, ba), (gb, bb) in zip(*out):
         assert torch.equal(ga, gb)
-        # the threshold is min(mean of the positive cells, thr) and the mean is a float atomicAdd reduction over millions of
-        # cells (order-dependent in its last bits): cells within ~1e-6 of it may flip, here and between any two runs
-        flipped = int(sum((((ba ^ bb).to(torch.int32) >> k) & 1).sum() for k in range(8)))
-        assert flipped <= 1e-4 * ga.numel()
+        # the threshold is min(mean of the positive cells, thr), and that mean is summed in a fixed order (k_grid_merge's
+        # per-block partials, added up by k_grid_mean): equal grids give equal bitfields
+        assert torch.equal(ba, bb)
