@@ -155,7 +155,7 @@ typedef struct {
     const float* ts;
     int64_t n;            /* number of samples, or the CAPACITY when n_dev is set */
     const int32_t* n_dev; /* optional device int32: the kernels read the sample count from here (no host sync) */
-    /* backward only (ngp_net_backward*, default kernel with feat_save): visit just the samples live_idx[0 .. *n_live_dev),
+    /* backward only (ngp_net_backward*; a live list needs feat_save): visit just the samples live_idx[0 .. *n_live_dev),
      * i.e. those whose upstream gradient can be non-zero -- the samples past a ray's termination receive exactly
      * zero gradient from composite_train_bw (volumerendering.cu:87-151) and contribute +0 to every sum. NULL = all. */
     const int32_t* live_idx;

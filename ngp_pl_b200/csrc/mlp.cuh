@@ -116,8 +116,7 @@ __device__ __forceinline__ void relu_bwd_to_frag(const float (&dC)[MT][N / 8][4]
 }
 
 // ---- shared-memory weight block -----------------------------------------------------------------
-// forward operands W[out][in] (+8 halfs of row padding), and for the backward the transposes
-// WT[in][out] (+8) that serve as B operands of the dgrad GEMMs.
+// operands W[out][in] (+8 halfs of row padding); the backward reads the same block (mlp_layer_dgrad).
 #define LD32 40
 #define LD64 72
 #define LD16 24
@@ -127,13 +126,6 @@ struct MlpWeightsFwd {
     __half w1r[64 * LD32];  // rgb 32 -> 64
     __half w2r[64 * LD64];  // rgb 64 -> 64
     __half w3r[16 * LD64];  // rgb 64 -> 16 (3 used)
-};
-struct MlpWeightsBwd {
-    __half w1dT[32 * LD64];  // [in=32][out=64]
-    __half w2dT[64 * LD16];  // [in=64][out=16]
-    __half w1rT[32 * LD64];
-    __half w2rT[64 * LD64];
-    __half w3rT[64 * LD16];
 };
 
 // Row-major [rows][cols] global matrix -> padded shared rows, 16 bytes per cp.async (cols % 8 == 0, ld % 8 == 0, both
@@ -152,11 +144,6 @@ __device__ __forceinline__ void load_matrix(__half* dst, int ld, const __half* _
         cp_async_16(dst + r * ld + 8 * c, src + r * cols + 8 * c);
     }
 }
-__device__ __forceinline__ void load_matrix_T(__half* dst, int ld, const __half* __restrict__ src, int rows, int cols,
-                                              int tid, int nthreads) {
-    // dst[c][r] = src[r][c]
-    for (int i = tid; i < rows * cols; i += nthreads) dst[(i % cols) * ld + (i / cols)] = src[i];
-}
 __device__ __forceinline__ void load_weights_fwd(MlpWeightsFwd& s, const __half* __restrict__ wd, const __half* __restrict__ wr,
                                                  int tid, int nthreads) {
     load_matrix(s.w1d, LD32, wd, 64, 32, tid, nthreads);
@@ -167,14 +154,6 @@ __device__ __forceinline__ void load_weights_fwd(MlpWeightsFwd& s, const __half*
         load_matrix(s.w3r, LD64, wr + 2048 + 4096, 16, 64, tid, nthreads);
     }
     cp_async_wait_all();
-}
-__device__ __forceinline__ void load_weights_bwd(MlpWeightsBwd& s, const __half* __restrict__ wd, const __half* __restrict__ wr,
-                                                 int tid, int nthreads) {
-    load_matrix_T(s.w1dT, LD64, wd, 64, 32, tid, nthreads);
-    load_matrix_T(s.w2dT, LD16, wd + 2048, 16, 64, tid, nthreads);
-    load_matrix_T(s.w1rT, LD64, wr, 64, 32, tid, nthreads);
-    load_matrix_T(s.w2rT, LD64, wr + 2048, 64, 64, tid, nthreads);
-    load_matrix_T(s.w3rT, LD16, wr + 2048 + 4096, 16, 64, tid, nthreads);
 }
 
 // ldmatrix with transpose: four 8x8 b16 tiles; lane l supplies the address of row (l&7) of tile (l>>3).
@@ -189,7 +168,7 @@ __device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, co
     asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];\n" : "=r"(r0), "=r"(r1) : "r"(a));
 }
 
-// ---- pieces of the layer-sequential backward (k_ngp_bwd2) -------------------------------------------
+// ---- backward (network.cu: k_ngp_bwd3, modules.cu) ------------------------------------------------
 
 // dX[16 x N] = dY[16 x K] * W[K rows (out)][N cols (in)]  with W row-major (LD halfs per row) in shared
 // memory: the B fragments (k = out row, n = in column) are the TRANSPOSE of what a plain 32-bit load of
@@ -212,19 +191,5 @@ __device__ __forceinline__ void mlp_layer_dgrad(const uint32_t (&A)[1][K / 16][4
             mma_16816(C[0][j], A[0][kt], b[0], b[1]);
             mma_16816(C[0][j + 1], A[0][kt], b[2], b[3]);
         }
-    }
-}
-
-// A fragments of 16 rows read back from a [row][channel] shared-memory tile (inverse of stage_frag)
-template <int KT>
-__device__ __forceinline__ void load_frag(const __half* __restrict__ src, int ld, int row0, uint32_t (&A)[1][KT][4], int g, int q) {
-#pragma unroll
-    for (int kt = 0; kt < KT; ++kt) {
-        const uint32_t* r0 = reinterpret_cast<const uint32_t*>(src + (row0 + g) * ld + 16 * kt + 2 * q);
-        const uint32_t* r1 = reinterpret_cast<const uint32_t*>(src + (row0 + g + 8) * ld + 16 * kt + 2 * q);
-        A[0][kt][0] = r0[0];
-        A[0][kt][1] = r1[0];
-        A[0][kt][2] = r0[4];
-        A[0][kt][3] = r1[4];
     }
 }

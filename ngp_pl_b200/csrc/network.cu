@@ -9,7 +9,6 @@
 #include "wgmma.cuh"
 #include "../../include/ngp_b200.h"
 #include <math.h>
-#include <stdlib.h>
 
 extern "C" int ngp_abi_version(void) { return NGP_ABI_VERSION; }
 
@@ -233,8 +232,10 @@ __device__ __forceinline__ float hi_half(uint32_t u) { return __half2float(__ush
 // -------------------------------------------------------------------------------------------------
 // forward
 // -------------------------------------------------------------------------------------------------
-template <int FWD_MT, int FWD_THREADS, int MIN_BLOCKS>
-__global__ void __launch_bounds__(FWD_THREADS, MIN_BLOCKS)
+#define FWD_MT 1            // 16-row tiles a warp takes at a time
+#define FWD_THREADS 256
+#define FWD_MIN_BLOCKS 3    // CTAs per SM: 24 warps
+__global__ void __launch_bounds__(FWD_THREADS, FWD_MIN_BLOCKS)
 k_ngp_fwd(const NgpNet net, const NgpSamples smp, const int want_rgb, float* __restrict__ sigmas, float* __restrict__ rgbs,
           __half* __restrict__ h_out, uint4* __restrict__ feat_save, int* __restrict__ sched) {
     __shared__ __align__(16) MlpWeightsFwd sw;
@@ -358,651 +359,38 @@ k_ngp_fwd(const NgpNet net, const NgpSamples smp, const int want_rgb, float* __r
     sched_finish(sched);
 }
 
-template <int MT, int THREADS, int MIN_BLOCKS>
-static int launch_fwd(const NgpNet* net, const NgpSamples* smp, int want_rgb, float* sigmas, float* rgbs, uint16_t* h_out,
-                      void* feat_save, cudaStream_t st) {
-    const int64_t n_tiles = (smp->n + 16 * MT - 1) / (16 * MT);
-    const int64_t want = (n_tiles + THREADS / 32 - 1) / (THREADS / 32);
-    const int64_t cap = (int64_t)ngp_sm_count() * MIN_BLOCKS;
-    const int grid = (int)(want < cap ? want : cap);
-    int* sched = sched_slot(st);
-    k_ngp_fwd<MT, THREADS, MIN_BLOCKS><<<grid, THREADS, 0, st>>>(*net, *smp, want_rgb, sigmas, rgbs, (__half*)h_out,
-                                                                 (uint4*)feat_save, sched);
-    return 0;
-}
-
-// NGP_FWD_VARIANT (env, read once) selects the tile/occupancy variant; the default is the measured best.
-static int fwd_variant() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("NGP_FWD_VARIANT");
-        v = e ? atoi(e) : 3;
-    }
-    return v;
-}
-
 extern "C" int ngp_net_forward(const NgpNet* net, const NgpSamples* smp, int want_rgb, float* sigmas, float* rgbs,
                                uint16_t* h_out, void* feat_save, void* stream) {
     if (!net || !smp || smp->n < 0 || !sigmas || (want_rgb && !rgbs)) return NGP_EINVAL;
     if (net->meta.n_levels < 1 || net->meta.n_levels > NGP_MAX_LEVELS) return NGP_EINVAL;
     if (smp->n == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    switch (fwd_variant()) {
-        case 0: launch_fwd<2, 256, 1>(net, smp, want_rgb, sigmas, rgbs, h_out, feat_save, st); break;   // 32 samples/warp, 8 warps/SM
-        case 2: launch_fwd<1, 128, 5>(net, smp, want_rgb, sigmas, rgbs, h_out, feat_save, st); break;   // 16 samples/warp, 20 warps/SM
-        case 3: launch_fwd<1, 256, 3>(net, smp, want_rgb, sigmas, rgbs, h_out, feat_save, st); break;   // 16 samples/warp, 24 warps/SM
-        default: launch_fwd<1, 256, 2>(net, smp, want_rgb, sigmas, rgbs, h_out, feat_save, st); break;  // 16 samples/warp, 16 warps/SM
-    }
+    const int64_t n_tiles = (smp->n + 16 * FWD_MT - 1) / (16 * FWD_MT);
+    const int64_t want = (n_tiles + FWD_THREADS / 32 - 1) / (FWD_THREADS / 32);
+    const int64_t cap = (int64_t)ngp_sm_count() * FWD_MIN_BLOCKS;
+    const int grid = (int)(want < cap ? want : cap);
+    k_ngp_fwd<<<grid, FWD_THREADS, 0, st>>>(*net, *smp, want_rgb, sigmas, rgbs, (__half*)h_out, (uint4*)feat_save,
+                                            sched_slot(st));
     NGP_CHECK_LAUNCH();
     NGP_TRACE(3, st);
     return 0;
 }
 
 // -------------------------------------------------------------------------------------------------
-// backward
-// -------------------------------------------------------------------------------------------------
-#define BWD_WARPS 8
-#define BWD_THREADS (BWD_WARPS * 32)
-#define BWD_ROWS (BWD_WARPS * 16)
-
-// per-CTA staging of the operands of the five weight-gradient GEMMs, [sample][channel] fp16
-struct BwdStage {
-    __half feat[BWD_ROWS * LD32];  // in  of W1d
-    __half hid[BWD_ROWS * LD64];   // in  of W2d
-    __half rin[BWD_ROWS * LD32];   // in  of W1r
-    __half r1[BWD_ROWS * LD64];    // in  of W2r
-    __half r2[BWD_ROWS * LD64];    // in  of W3r
-    __half dhid[BWD_ROWS * LD64];  // out-grad of W1d
-    __half dh[BWD_ROWS * LD16];    // out-grad of W2d
-    __half dr1[BWD_ROWS * LD64];   // out-grad of W1r
-    __half dr2[BWD_ROWS * LD64];   // out-grad of W2r
-    __half dout[BWD_ROWS * LD16];  // out-grad of W3r
-};
-struct BwdSmem {
-    MlpWeightsFwd wf;
-    MlpWeightsBwd wb;
-    BwdStage st;
-};
-
-template <int KT>
-__device__ __forceinline__ void stage_frag(__half* __restrict__ dst, int ld, int row0, const uint32_t (&A)[KT][4], int g, int q) {
-#pragma unroll
-    for (int kt = 0; kt < KT; ++kt) {
-        uint32_t* r0 = reinterpret_cast<uint32_t*>(dst + (row0 + g) * ld + 16 * kt + 2 * q);
-        uint32_t* r1 = reinterpret_cast<uint32_t*>(dst + (row0 + g + 8) * ld + 16 * kt + 2 * q);
-        r0[0] = A[kt][0];
-        r1[0] = A[kt][1];
-        r0[4] = A[kt][2];
-        r1[4] = A[kt][3];
-    }
-}
-
-// one 16x8 tile of dW = dOut^T * In accumulated over the BWD_ROWS staged samples
-__device__ __forceinline__ void wgrad_tile(float (&acc)[4], const __half* __restrict__ dOut, int ld_o, int mt,
-                                           const __half* __restrict__ In, int ld_i, int nt, int lane) {
-    const int ra = (lane & 7) + 8 * ((lane >> 4) & 1);  // sample row inside the 16-row k-step (A operand tiles)
-    const int ca = 16 * mt + 8 * ((lane >> 3) & 1);     // out-channel column of the tile this lane addresses
-    const int rb = (lane & 7) + 8 * ((lane >> 3) & 1);  // sample row for the two B tiles
-    const int cb = 8 * nt;
-#pragma unroll
-    for (int ks = 0; ks < BWD_ROWS / 16; ++ks) {
-        uint32_t a[4], b0, b1;
-        ldmatrix_x4_trans(a, dOut + (16 * ks + ra) * ld_o + ca);
-        ldmatrix_x2_trans(b0, b1, In + (16 * ks + rb) * ld_i + cb);
-        mma_16816(acc, a, b0, b1);
-    }
-}
-
-__device__ __forceinline__ void wgrad_flush(const float (&acc)[4], float* __restrict__ dW, int in_dim, int mt, int nt,
-                                            float inv_scale, int g, int q) {
-    float* p0 = dW + (16 * mt + g) * in_dim + 8 * nt + 2 * q;
-    float* p1 = dW + (16 * mt + g + 8) * in_dim + 8 * nt + 2 * q;
-    red_add_f32x2(p0, acc[0] * inv_scale, acc[1] * inv_scale);
-    red_add_f32x2(p1, acc[2] * inv_scale, acc[3] * inv_scale);
-}
-
-// wgrad tile table: 80 (matrix, out-tile, in-tile) triples, 10 per warp
-struct WgradTile {
-    int mat, mt, nt;
-};
-__device__ __forceinline__ WgradTile wgrad_tile_of(int t) {
-    WgradTile w;
-    if (t < 16) { w.mat = 0; w.mt = t >> 2; w.nt = t & 3; }                 // dW1d 64x32
-    else if (t < 24) { w.mat = 1; w.mt = 0; w.nt = t - 16; }                // dW2d 16x64
-    else if (t < 40) { w.mat = 2; w.mt = (t - 24) >> 2; w.nt = (t - 24) & 3; }  // dW1r 64x32
-    else if (t < 72) { w.mat = 3; w.mt = (t - 40) >> 3; w.nt = (t - 40) & 7; }  // dW2r 64x64
-    else { w.mat = 4; w.mt = 0; w.nt = t - 72; }                            // dW3r 16x64
-    return w;
-}
-
-__global__ void __launch_bounds__(BWD_THREADS, 1)
-k_ngp_bwd(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_dsigmas, const float* __restrict__ dL_drgbs,
-          const uint4* __restrict__ feat_save, const float* __restrict__ loss_scale, float* __restrict__ grad_enc,
-          float* __restrict__ grad_rgb, uint32_t* __restrict__ dfeat, const int64_t dfeat_stride) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    BwdSmem& S = *reinterpret_cast<BwdSmem*>(smem_raw);
-    const __half* wd = reinterpret_cast<const __half*>(net.enc_params_h);
-    const __half* wr = reinterpret_cast<const __half*>(net.rgb_params_h);
-    load_weights_fwd(S.wf, wd, wr, threadIdx.x, BWD_THREADS);
-    load_weights_bwd(S.wb, wd, wr, threadIdx.x, BWD_THREADS);
-    __syncthreads();
-    const uint32_t* table = reinterpret_cast<const uint32_t*>(wd + NGP_DENSITY_MLP_PARAMS);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
-    const int64_t n = sample_count(smp);
-    const int64_t n_mtiles = (n + 15) / 16;
-    const int64_t n_blks = (n_mtiles + BWD_WARPS - 1) / BWD_WARPS;
-    const float scale = loss_scale ? *loss_scale : 1.0f;
-    const float inv_scale = 1.0f / scale;
-
-    float acc[10][4];
-#pragma unroll
-    for (int j = 0; j < 10; ++j)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
-
-    for (int64_t blk = blockIdx.x; blk < n_blks; blk += gridDim.x) {
-        const int64_t mtile = blk * BWD_WARPS + warp;
-        const int64_t base = mtile * 16;
-        SampleIn sm[1][2];
-        bool valid[1][2];
-        float u[1][2][3];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int64_t row = base + g + 8 * h;
-            valid[0][h] = row < n;
-            sm[0][h] = load_sample(smp, row, valid[0][h]);
-            to_unit(net, sm[0][h], u[0][h][0], u[0][h][1], u[0][h][2]);
-        }
-
-        // upstream gradients of this lane's rows: issued now, consumed after the forward recompute
-        float up_sig[2] = {0.f, 0.f}, up_c0[2] = {0.f, 0.f}, up_c1[2] = {0.f, 0.f};
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int64_t row = base + g + 8 * h;
-            if (valid[0][h]) {
-                if (q == 0) {
-                    up_sig[h] = __ldg(dL_dsigmas + row);
-                    up_c0[h] = __ldg(dL_drgbs + 3 * row);
-                    up_c1[h] = __ldg(dL_drgbs + 3 * row + 1);
-                } else if (q == 1) {
-                    up_c0[h] = __ldg(dL_drgbs + 3 * row + 2);
-                }
-            }
-        }
-
-        // ---- recompute the forward activations ----
-        uint32_t featA[1][2][4];
-        if (feat_save && base < n) {
-#pragma unroll
-            for (int kt = 0; kt < 2; ++kt) {
-                const uint4 v = __ldg(feat_save + (mtile * 2 + kt) * 32 + lane);
-                featA[0][kt][0] = v.x; featA[0][kt][1] = v.y; featA[0][kt][2] = v.z; featA[0][kt][3] = v.w;
-            }
-        } else {
-            encode_rows<1>(net, table, u, valid, featA, q);
-        }
-        uint32_t hidA[1][4][4];
-        {
-            float c[1][8][4];
-            mlp_layer<1, 32, 64, LD32>(featA, S.wf.w1d, c, g, q);
-            relu_to_frag<1, 64>(c, hidA);
-        }
-        uint32_t hA[1][1][4];
-        {
-            float c[1][2][4];
-            mlp_layer<1, 64, 16, LD64>(hidA, S.wf.w2d, c, g, q);
-            to_frag<1, 16>(c, hA);
-        }
-        uint32_t inA[1][2][4];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) sh_rows(sm[0][h], q, inA[0][0][h], inA[0][0][2 + h]);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) inA[0][1][e] = hA[0][0][e];
-        uint32_t r1A[1][4][4];
-        {
-            float c[1][8][4];
-            mlp_layer<1, 32, 64, LD32>(inA, S.wf.w1r, c, g, q);
-            relu_to_frag<1, 64>(c, r1A);
-        }
-        uint32_t r2A[1][4][4];
-        {
-            float c[1][8][4];
-            mlp_layer<1, 64, 64, LD64>(r1A, S.wf.w2r, c, g, q);
-            relu_to_frag<1, 64>(c, r2A);
-        }
-        float oC[1][1][4];
-        mlp_layer<1, 64, 8, LD64>(r2A, S.wf.w3r, oC, g, q);
-
-        // ---- output gradients (scaled by the power-of-two loss scale before the fp16 cast) ----
-        uint32_t doutA[1][1][4];
-        doutA[0][0][2] = 0u;
-        doutA[0][0][3] = 0u;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int64_t row = base + g + 8 * h;
-            float d0 = 0.f, d1 = 0.f;
-            if (valid[0][h] && q < 2) {
-                float o0 = oC[0][0][2 * h], o1 = oC[0][0][2 * h + 1];
-                float s0 = 1.f, s1 = 1.f;
-                if (net.rgb_act == 1) {
-                    o0 = half_round(1.0f / (1.0f + __expf(-o0)));
-                    o1 = half_round(1.0f / (1.0f + __expf(-o1)));
-                    s0 = o0 * (1.0f - o0);
-                    s1 = o1 * (1.0f - o1);
-                }
-                d0 = up_c0[h] * s0 * scale;
-                d1 = (q == 0) ? up_c1[h] * s1 * scale : 0.f;
-            }
-            doutA[0][0][h] = pack_half2(d0, d1);
-        }
-
-        // ---- dgrad chain of the rgb net ----
-        uint32_t dr2A[1][4][4];
-        {
-            float c[1][8][4];
-            mlp_layer<1, 16, 64, LD16>(doutA, S.wb.w3rT, c, g, q);
-            relu_bwd_to_frag<1, 64>(c, r2A, dr2A);
-        }
-        uint32_t dr1A[1][4][4];
-        {
-            float c[1][8][4];
-            mlp_layer<1, 64, 64, LD64>(dr2A, S.wb.w2rT, c, g, q);
-            relu_bwd_to_frag<1, 64>(c, r1A, dr1A);
-        }
-        // gradient w.r.t. the h half of the rgb-net input (columns 16..31); SH columns need no gradient
-        uint32_t dhA[1][1][4];
-        {
-            float c[1][2][4];
-            mlp_layer<1, 64, 16, LD64>(dr1A, S.wb.w1rT + 16 * LD64, c, g, q);
-            // + density branch: d sigma / d h0 = exp(clamp(h0, -15, 15))  (reference custom_functions.py:169-173)
-            if (q == 0) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int64_t row = base + g + 8 * h;
-                    if (valid[0][h]) {
-                        const float h0 = lo_half(hA[0][0][h]);
-                        c[0][0][2 * h] += up_sig[h] * expf(fminf(fmaxf(h0, -15.f), 15.f)) * scale;
-                    }
-                }
-            }
-            to_frag<1, 16>(c, dhA);
-        }
-        uint32_t dhidA[1][4][4];
-        {
-            float c[1][8][4];
-            mlp_layer<1, 16, 64, LD16>(dhA, S.wb.w2dT, c, g, q);
-            relu_bwd_to_frag<1, 64>(c, hidA, dhidA);
-        }
-        // ---- gradient of the encoded features (still multiplied by the loss scale), stored [level][sample] as
-        //      half2 for the scatter kernel: lanes with equal q write 8 consecutive samples = one full sector ----
-        {
-            float c[1][4][4];
-            mlp_layer<1, 64, 32, LD64>(dhidA, S.wb.w1dT, c, g, q);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int64_t row = base + g + 8 * h;
-                if (!valid[0][h]) continue;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int level = 4 * j + q;
-                    if (level < net.meta.n_levels)
-                        dfeat[(int64_t)level * dfeat_stride + row] = pack_half2(c[0][j][2 * h], c[0][j][2 * h + 1]);
-                }
-            }
-        }
-
-        // ---- stage the wgrad operands and run the five dW GEMMs over this CTA's 128 samples ----
-        const int row0 = 16 * warp;
-        stage_frag<2>(S.st.feat, LD32, row0, featA[0], g, q);
-        stage_frag<4>(S.st.hid, LD64, row0, hidA[0], g, q);
-        stage_frag<2>(S.st.rin, LD32, row0, inA[0], g, q);
-        stage_frag<4>(S.st.r1, LD64, row0, r1A[0], g, q);
-        stage_frag<4>(S.st.r2, LD64, row0, r2A[0], g, q);
-        stage_frag<4>(S.st.dhid, LD64, row0, dhidA[0], g, q);
-        stage_frag<1>(S.st.dh, LD16, row0, dhA[0], g, q);
-        stage_frag<4>(S.st.dr1, LD64, row0, dr1A[0], g, q);
-        stage_frag<4>(S.st.dr2, LD64, row0, dr2A[0], g, q);
-        stage_frag<1>(S.st.dout, LD16, row0, doutA[0], g, q);
-        __syncthreads();
-#pragma unroll
-        for (int j = 0; j < 10; ++j) {
-            const WgradTile w = wgrad_tile_of(warp * 10 + j);
-            const __half* dO; const __half* In; int ldo, ldi;
-            switch (w.mat) {
-                case 0: dO = S.st.dhid; ldo = LD64; In = S.st.feat; ldi = LD32; break;
-                case 1: dO = S.st.dh; ldo = LD16; In = S.st.hid; ldi = LD64; break;
-                case 2: dO = S.st.dr1; ldo = LD64; In = S.st.rin; ldi = LD32; break;
-                case 3: dO = S.st.dr2; ldo = LD64; In = S.st.r1; ldi = LD64; break;
-                default: dO = S.st.dout; ldo = LD16; In = S.st.r2; ldi = LD64; break;
-            }
-            wgrad_tile(acc[j], dO, ldo, w.mt, In, ldi, w.nt, lane);
-        }
-        __syncthreads();
-    }
-
-    // ---- flush the per-warp weight-gradient tiles ----
-#pragma unroll
-    for (int j = 0; j < 10; ++j) {
-        const WgradTile w = wgrad_tile_of(warp * 10 + j);
-        switch (w.mat) {
-            case 0: wgrad_flush(acc[j], grad_enc, 32, w.mt, w.nt, inv_scale, g, q); break;
-            case 1: wgrad_flush(acc[j], grad_enc + 2048, 64, w.mt, w.nt, inv_scale, g, q); break;
-            case 2: wgrad_flush(acc[j], grad_rgb, 32, w.mt, w.nt, inv_scale, g, q); break;
-            case 3: wgrad_flush(acc[j], grad_rgb + 2048, 64, w.mt, w.nt, inv_scale, g, q); break;
-            default: wgrad_flush(acc[j], grad_rgb + 2048 + 4096, 64, w.mt, w.nt, inv_scale, g, q); break;
-        }
-    }
-}
-
-// -------------------------------------------------------------------------------------------------
-// backward, layer-sequential variant (default): 16 warps per CTA instead of 8, <= 128 registers.
-// The recomputed activations are staged to shared memory as they are produced (they are the `In`
-// operands of the weight-gradient GEMMs anyway) instead of being held in registers until the end; one
-// out-gradient buffer is reused layer after layer:   stage dOut -> sync -> {wgrad tiles of this layer
-// (every warp reads all 256 staged rows), dgrad of this layer (own rows, B fragments by ldmatrix.trans from
-// the forward weights)} -> sync -> next layer.   80 wgrad tiles / 16 warps = 5 accumulator tiles per warp.
-// -------------------------------------------------------------------------------------------------
-#define B2_WARPS 16
-#define B2_THREADS (B2_WARPS * 32)
-#define B2_ROWS (B2_WARPS * 16)
-struct Bwd2Smem {
-    MlpWeightsFwd wf;
-    __half feat[B2_ROWS * LD32];
-    __half hid[B2_ROWS * LD64];
-    __half rin[B2_ROWS * LD32];
-    __half r1[B2_ROWS * LD64];
-    __half r2[B2_ROWS * LD64];
-    __half dout[B2_ROWS * LD64];  // out-gradient of the layer being processed
-};
-
-// one 16x8 tile of dW accumulated over the B2_ROWS staged samples
-__device__ __forceinline__ void wgrad_tile2(float (&acc)[4], const __half* __restrict__ dOut, int ld_o, int mt,
-                                            const __half* __restrict__ In, int ld_i, int nt, int lane) {
-    const int ra = (lane & 7) + 8 * ((lane >> 4) & 1);
-    const int ca = 16 * mt + 8 * ((lane >> 3) & 1);
-    const int rb = (lane & 7) + 8 * ((lane >> 3) & 1);
-    const int cb = 8 * nt;
-#pragma unroll 4
-    for (int ks = 0; ks < B2_ROWS / 16; ++ks) {
-        uint32_t a[4], b0, b1;
-        ldmatrix_x4_trans(a, dOut + (16 * ks + ra) * ld_o + ca);
-        ldmatrix_x2_trans(b0, b1, In + (16 * ks + rb) * ld_i + cb);
-        mma_16816(acc, a, b0, b1);
-    }
-}
-// two tiles sharing the dOut operand (same out-tile, neighbouring in-tiles)
-__device__ __forceinline__ void wgrad_tile2x2(float (&acc0)[4], float (&acc1)[4], const __half* __restrict__ dOut, int ld_o,
-                                              int mt, const __half* __restrict__ In, int ld_i, int nt, int lane) {
-    const int ra = (lane & 7) + 8 * ((lane >> 4) & 1);
-    const int ca = 16 * mt + 8 * ((lane >> 3) & 1);
-    const int rb = (lane & 7) + 8 * ((lane >> 3) & 1);
-    const int cb = 8 * nt + 8 * (lane >> 4);
-#pragma unroll 4
-    for (int ks = 0; ks < B2_ROWS / 16; ++ks) {
-        uint32_t a[4], b[4];
-        ldmatrix_x4_trans(a, dOut + (16 * ks + ra) * ld_o + ca);
-        ldmatrix_x4_trans(b, In + (16 * ks + rb) * ld_i + cb);
-        mma_16816(acc0, a, b[0], b[1]);
-        mma_16816(acc1, a, b[2], b[3]);
-    }
-}
-
-__global__ void __launch_bounds__(B2_THREADS, 1)
-k_ngp_bwd2(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_dsigmas, const float* __restrict__ dL_drgbs,
-           const uint4* __restrict__ feat_save, const float* __restrict__ loss_scale, float* __restrict__ grad_enc,
-           float* __restrict__ grad_rgb, uint32_t* __restrict__ dfeat, const int64_t dfeat_stride, int* __restrict__ sched) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    Bwd2Smem& S = *reinterpret_cast<Bwd2Smem*>(smem_raw);
-    __shared__ int s_blk[2];  // tickets of the current and the next block of 256 rows (double-buffered)
-    const __half* wd = reinterpret_cast<const __half*>(net.enc_params_h);
-    const __half* wr = reinterpret_cast<const __half*>(net.rgb_params_h);
-    load_weights_fwd(S.wf, wd, wr, threadIdx.x, B2_THREADS);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
-    const int64_t n = bwd_count(smp);
-    const int32_t* __restrict__ live = smp.live_idx;
-    const int64_t n_mtiles = (n + 15) / 16;
-    const int64_t n_blks = (n_mtiles + B2_WARPS - 1) / B2_WARPS;
-    const float scale = loss_scale ? *loss_scale : 1.0f;
-    const float inv_scale = 1.0f / scale;
-    const int row0 = 16 * warp;
-    const int wm = warp >> 2, wn = warp & 3;  // (out-tile, in-tile) role of this warp in the 16-tile GEMMs
-
-    // accumulators: [0] W3r (warps 0-7) or W2d (warps 8-15), [1],[2] W2r, [3] W1r, [4] W1d
-    float acc[5][4];
-#pragma unroll
-    for (int j = 0; j < 5; ++j)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
-
-    if (threadIdx.x == 0) s_blk[0] = sched ? atomicAdd(&sched[0], 1) : (int)blockIdx.x;
-    __syncthreads();
-    for (int it = 0;; ++it) {
-        const int64_t blk = s_blk[it & 1];
-        if (blk >= n_blks) break;
-        // ticket of the next block: written to the other slot, published by this iteration's barriers
-        if (threadIdx.x == 0) s_blk[(it + 1) & 1] = sched ? atomicAdd(&sched[0], 1) : (int)(blk + gridDim.x);
-        const int64_t mtile = blk * B2_WARPS + warp;
-        const int64_t base = mtile * 16;
-        bool valid[2];
-        float up_sig[2] = {0.f, 0.f}, up_c0[2] = {0.f, 0.f}, up_c1[2] = {0.f, 0.f};
-        SampleIn sm[2];
-        int64_t src[2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int64_t row = base + g + 8 * h;
-            valid[h] = row < n;
-            src[h] = valid[h] ? (live ? (int64_t)__ldg(live + row) : row) : 0;
-            sm[h] = load_sample(smp, src[h], valid[h]);
-            if (valid[h]) {
-                if (q == 0) {
-                    up_sig[h] = __ldg(dL_dsigmas + src[h]);
-                    up_c0[h] = __ldg(dL_drgbs + 3 * src[h]);
-                    up_c1[h] = __ldg(dL_drgbs + 3 * src[h] + 1);
-                } else if (q == 1) {
-                    up_c0[h] = __ldg(dL_drgbs + 3 * src[h] + 2);
-                }
-            }
-        }
-        uint32_t featA[1][2][4];
-        if (live) {
-            // rows come from arbitrary forward tiles: pick this lane's four words of each row out of the forward's
-            // fragment-order save (word x/z = row g, y/w = row g+8 of the tile that holds the sample)
-            const uint32_t* fs = reinterpret_cast<const uint32_t*>(feat_save);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int64_t t2 = (src[h] >> 4) * 2;
-                const int r = (int)(src[h] & 15);
-                const int64_t w0 = (r & 7) * 4 + q;
-                const int sub = r >> 3;
-#pragma unroll
-                for (int kt = 0; kt < 2; ++kt) {
-                    const uint32_t* p = fs + ((t2 + kt) * 32 + w0) * 4 + sub;
-                    featA[0][kt][h] = valid[h] ? __ldg(p) : 0u;
-                    featA[0][kt][2 + h] = valid[h] ? __ldg(p + 2) : 0u;
-                }
-            }
-        } else if (base < n) {
-#pragma unroll
-            for (int kt = 0; kt < 2; ++kt) {
-                const uint4 v = __ldg(feat_save + (mtile * 2 + kt) * 32 + lane);
-                featA[0][kt][0] = v.x; featA[0][kt][1] = v.y; featA[0][kt][2] = v.z; featA[0][kt][3] = v.w;
-            }
-        } else {
-#pragma unroll
-            for (int kt = 0; kt < 2; ++kt)
-#pragma unroll
-                for (int e = 0; e < 4; ++e) featA[0][kt][e] = 0u;
-        }
-        // every warp is done with the previous iteration's staged tensors (and, first time, the weights are loaded)
-        __syncthreads();
-
-        // ---- forward recompute, staging each activation as soon as it exists ----
-        stage_frag<2>(S.feat, LD32, row0, featA[0], g, q);
-        float h0[2];
-        uint32_t hA[1][1][4];
-        {
-            uint32_t hidA[1][4][4];
-            {
-                float c[1][8][4];
-                mlp_layer<1, 32, 64, LD32>(featA, S.wf.w1d, c, g, q);
-                relu_to_frag<1, 64>(c, hidA);
-            }
-            stage_frag<4>(S.hid, LD64, row0, hidA[0], g, q);
-            float c[1][2][4];
-            mlp_layer<1, 64, 16, LD64>(hidA, S.wf.w2d, c, g, q);
-            to_frag<1, 16>(c, hA);
-        }
-        h0[0] = lo_half(hA[0][0][0]);
-        h0[1] = lo_half(hA[0][0][1]);
-        uint32_t doutA[1][1][4];
-        {
-            uint32_t inA[1][2][4];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) sh_rows(sm[h], q, inA[0][0][h], inA[0][0][2 + h]);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) inA[0][1][e] = hA[0][0][e];
-            stage_frag<2>(S.rin, LD32, row0, inA[0], g, q);
-            uint32_t r1A[1][4][4];
-            {
-                float c[1][8][4];
-                mlp_layer<1, 32, 64, LD32>(inA, S.wf.w1r, c, g, q);
-                relu_to_frag<1, 64>(c, r1A);
-            }
-            stage_frag<4>(S.r1, LD64, row0, r1A[0], g, q);
-            uint32_t r2A[1][4][4];
-            {
-                float c[1][8][4];
-                mlp_layer<1, 64, 64, LD64>(r1A, S.wf.w2r, c, g, q);
-                relu_to_frag<1, 64>(c, r2A);
-            }
-            stage_frag<4>(S.r2, LD64, row0, r2A[0], g, q);
-            float oC[1][1][4];
-            mlp_layer<1, 64, 8, LD64>(r2A, S.wf.w3r, oC, g, q);
-            doutA[0][0][2] = 0u;
-            doutA[0][0][3] = 0u;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                float d0 = 0.f, d1 = 0.f;
-                if (valid[h] && q < 2) {
-                    float o0 = oC[0][0][2 * h], o1 = oC[0][0][2 * h + 1];
-                    float s0 = 1.f, s1 = 1.f;
-                    if (net.rgb_act == 1) {
-                        o0 = half_round(1.0f / (1.0f + __expf(-o0)));
-                        o1 = half_round(1.0f / (1.0f + __expf(-o1)));
-                        s0 = o0 * (1.0f - o0);
-                        s1 = o1 * (1.0f - o1);
-                    }
-                    d0 = up_c0[h] * s0 * scale;
-                    d1 = (q == 0) ? up_c1[h] * s1 * scale : 0.f;
-                }
-                doutA[0][0][h] = pack_half2(d0, d1);
-            }
-        }
-
-        // ---- layer rgb-3 : W3r (16 x 64) ----
-        stage_frag<1>(S.dout, LD64, row0, doutA[0], g, q);
-        __syncthreads();
-        if (warp < 8) wgrad_tile2(acc[0], S.dout, LD64, 0, S.r2, LD64, warp, lane);
-        uint32_t dA[1][4][4];  // out-gradient fragments of the 64-wide layers, reused
-        {
-            float c[1][8][4];
-            mlp_layer_dgrad<16, 64, LD64>(doutA, S.wf.w3r, c, lane);
-            uint32_t act[1][4][4];
-            load_frag<4>(S.r2, LD64, row0, act, g, q);
-            relu_bwd_to_frag<1, 64>(c, act, dA);
-        }
-        __syncthreads();
-
-        // ---- layer rgb-2 : W2r (64 x 64) ----
-        stage_frag<4>(S.dout, LD64, row0, dA[0], g, q);
-        __syncthreads();
-        wgrad_tile2x2(acc[1], acc[2], S.dout, LD64, wm, S.r1, LD64, 2 * wn, lane);
-        {
-            float c[1][8][4];
-            mlp_layer_dgrad<64, 64, LD64>(dA, S.wf.w2r, c, lane);
-            uint32_t act[1][4][4];
-            load_frag<4>(S.r1, LD64, row0, act, g, q);
-            relu_bwd_to_frag<1, 64>(c, act, dA);
-        }
-        __syncthreads();
-
-        // ---- layer rgb-1 : W1r (64 x 32); only the h half of its input needs a gradient ----
-        stage_frag<4>(S.dout, LD64, row0, dA[0], g, q);
-        __syncthreads();
-        wgrad_tile2(acc[3], S.dout, LD64, wm, S.rin, LD32, wn, lane);
-        uint32_t dhA[1][1][4];
-        {
-            float c[1][2][4];
-            mlp_layer_dgrad<64, 16, LD32>(dA, S.wf.w1r + 16, c, lane);
-            if (q == 0) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (valid[h]) c[0][0][2 * h] += up_sig[h] * expf(fminf(fmaxf(h0[h], -15.f), 15.f)) * scale;
-            }
-            to_frag<1, 16>(c, dhA);
-        }
-        __syncthreads();
-
-        // ---- layer density-2 : W2d (16 x 64) ----
-        stage_frag<1>(S.dout, LD64, row0, dhA[0], g, q);
-        __syncthreads();
-        if (warp >= 8) wgrad_tile2(acc[0], S.dout, LD64, 0, S.hid, LD64, warp - 8, lane);
-        {
-            float c[1][8][4];
-            mlp_layer_dgrad<16, 64, LD64>(dhA, S.wf.w2d, c, lane);
-            uint32_t act[1][4][4];
-            load_frag<4>(S.hid, LD64, row0, act, g, q);
-            relu_bwd_to_frag<1, 64>(c, act, dA);
-        }
-        __syncthreads();
-
-        // ---- layer density-1 : W1d (64 x 32) -> feature gradients ----
-        stage_frag<4>(S.dout, LD64, row0, dA[0], g, q);
-        __syncthreads();
-        wgrad_tile2(acc[4], S.dout, LD64, wm, S.feat, LD32, wn, lane);
-        {
-            float c[1][4][4];
-            mlp_layer_dgrad<64, 32, LD32>(dA, S.wf.w1d, c, lane);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int64_t row = base + g + 8 * h;
-                if (!valid[h]) continue;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int level = 4 * j + q;
-                    if (level < net.meta.n_levels)
-                        dfeat[(int64_t)level * dfeat_stride + row] = pack_half2(c[0][j][2 * h], c[0][j][2 * h + 1]);
-                }
-            }
-        }
-    }
-
-    sched_finish(sched);
-    // ---- flush the weight-gradient tiles ----
-    if (warp < 8) wgrad_flush(acc[0], grad_rgb + 2048 + 4096, 64, 0, warp, inv_scale, g, q);  // W3r
-    else wgrad_flush(acc[0], grad_enc + 2048, 64, 0, warp - 8, inv_scale, g, q);              // W2d
-    wgrad_flush(acc[1], grad_rgb + 2048, 64, wm, 2 * wn, inv_scale, g, q);                    // W2r
-    wgrad_flush(acc[2], grad_rgb + 2048, 64, wm, 2 * wn + 1, inv_scale, g, q);
-    wgrad_flush(acc[3], grad_rgb, 32, wm, wn, inv_scale, g, q);                               // W1r
-    wgrad_flush(acc[4], grad_enc, 32, wm, wn, inv_scale, g, q);                               // W1d
-}
-
-// -------------------------------------------------------------------------------------------------
-// backward, warpgroup-MMA variant (default): the dgrad chain stays on mma.sync fragments in twelve ROW warps, but the five
-// WEIGHT-GRADIENT GEMMs (dW = dOut^T * In over the 192 staged rows of a block: K = 192, M = 64, N <= 64) are issued by a
-// dedicated MMA WARPGROUP (warps 12-15) as wgmma.mma_async with both operands read from shared memory through matrix
-// descriptors and the fp32 accumulators in that warpgroup's registers (64 x 160, 80 a thread, alive for the CTA's whole
-// lifetime; k_ngp_bwd2 keeps 20 accumulator registers per row thread and spends 1,280 mma.sync + 2,560 ldmatrix per block on
-// them). The activations are staged in the canonical MN-major no-swizzle layout (wgmma.cuh); the out-gradient of a layer
-// goes to one of two buffers, so the tensor core can still be reading layer L's while the warps stage layer L+1's.
+// backward: the dgrad chain stays on mma.sync fragments in twelve ROW warps, but the five WEIGHT-GRADIENT GEMMs
+// (dW = dOut^T * In over the 192 staged rows of a block: K = 192, M = 64, N <= 64) are issued by a dedicated MMA WARPGROUP
+// (warps 12-15) as wgmma.mma_async with both operands read from shared memory through matrix descriptors and the fp32
+// accumulators in that warpgroup's registers (64 x 160, 80 a thread, alive for the CTA's whole lifetime). The activations
+// are staged in the canonical MN-major no-swizzle layout (wgmma.cuh); the out-gradient of a layer goes to one of two
+// buffers, so the tensor core can still be reading layer L's while the warps stage layer L+1's.
 // Synchronisation is by mbarriers, not CTA barriers: a row thread that has staged its rows of a layer ARRIVES on that
 // layer's `staged` barrier and carries on with its dgrad; the MMA warpgroup WAITS on it, issues the 12 wgmma of the layer's
 // GEMM, waits for them and arrives on the `done` barrier of the buffer they read, which row threads wait on only before they
 // overwrite that buffer two layers later. One CTA barrier per 192-row block is left (ticket broadcast + reuse of the
-// activation tiles); k_ngp_bwd2 has eleven. Twelve row warps: a 512-thread block keeps the 128 registers a thread the row
-// path needs without spilling (sixteen would leave 96).
+// activation tiles). Twelve row warps: a 512-thread block keeps the 128 registers a thread the row path needs without
+// spilling (sixteen would leave 96).
+// The encoded features come from the forward's feat_save or, with REGATHER (no feat_save), from the hash table again
+// through the forward's own encode_rows, so both give the same fp16 values.
 // -------------------------------------------------------------------------------------------------
 #define B3_WARPS 12
 #define B3_ROW_THREADS (B3_WARPS * 32)
@@ -1084,6 +472,7 @@ __device__ __forceinline__ void wgmma_acc_flush(const float (&d)[N / 2], float* 
         }
 }
 
+template <bool REGATHER>
 __global__ void __launch_bounds__(B3_THREADS, 1)
 k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_dsigmas, const float* __restrict__ dL_drgbs,
            const uint4* __restrict__ feat_save, const float* __restrict__ loss_scale, float* __restrict__ grad_enc,
@@ -1176,7 +565,6 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
         }
     };
     auto fetch_hop2 = [&](int64_t nblk) {  // everything that is indexed by the sample
-        const uint32_t* fs = reinterpret_cast<const uint32_t*>(feat_save);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int64_t sidx = pre_src[h];
@@ -1195,17 +583,20 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
                     pre_up[h][1] = __ldg(dL_drgbs + 3 * sidx + 2);
                 }
             }
-            // this lane's four words of the row out of the forward's fragment-order save (word x/z = row g, y/w = row g+8 of
-            // the 16-row tile that holds the sample)
-            const int64_t t2 = (sidx >> 4) * 2;
-            const int r = (int)(sidx & 15);
-            const int64_t w0 = (r & 7) * 4 + q;
-            const int sub = r >> 3;
+            if constexpr (!REGATHER) {
+                // this lane's four words of the row out of the forward's fragment-order save (word x/z = row g, y/w = row
+                // g+8 of the 16-row tile that holds the sample)
+                const uint32_t* fs = reinterpret_cast<const uint32_t*>(feat_save);
+                const int64_t t2 = (sidx >> 4) * 2;
+                const int r = (int)(sidx & 15);
+                const int64_t w0 = (r & 7) * 4 + q;
+                const int sub = r >> 3;
 #pragma unroll
-            for (int kt = 0; kt < 2; ++kt) {
-                const uint32_t* p = fs + ((t2 + kt) * 32 + w0) * 4 + sub;
-                pre_feat[kt][h] = pre_valid[h] ? __ldg(p) : 0u;
-                pre_feat[kt][2 + h] = pre_valid[h] ? __ldg(p + 2) : 0u;
+                for (int kt = 0; kt < 2; ++kt) {
+                    const uint32_t* p = fs + ((t2 + kt) * 32 + w0) * 4 + sub;
+                    pre_feat[kt][h] = pre_valid[h] ? __ldg(p) : 0u;
+                    pre_feat[kt][2 + h] = pre_valid[h] ? __ldg(p + 2) : 0u;
+                }
             }
         }
         (void)nblk;
@@ -1255,6 +646,14 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
                 sm[h] = load_sample(smp, pre_src[h], v);  // (xyzs / dirs layout, or an invalid row)
                 valid[h] = v;
             }
+        }
+        if constexpr (REGATHER) {
+            const uint32_t* table = reinterpret_cast<const uint32_t*>(wd + NGP_DENSITY_MLP_PARAMS);
+            const bool v[1][2] = {{valid[0], valid[1]}};
+            float u[1][2][3];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) to_unit(net, sm[h], u[0][h][0], u[0][h][1], u[0][h][2]);
+            encode_rows<1>(net, table, u, v, featA, q);
         }
         // the previous block's GEMMs still read feat / hid / rin / r1 / r2: its last batch (W1d, buffer 0) completes after
         // every earlier one (the MMAs of one thread complete in order). The CTA barrier also publishes the next ticket and
@@ -1522,6 +921,7 @@ extern "C" int ngp_net_backward_mlp(const NgpNet* net, const NgpSamples* smp, co
     int rc = check_bwd_args(net, smp, workspace, workspace_bytes);
     if (rc) return rc;
     if (!dL_dsigmas || !dL_drgbs || !grad_enc || !grad_rgb) return NGP_EINVAL;
+    if (smp->live_idx && (!smp->n_live_dev || !feat_save)) return NGP_EINVAL;  // a live list needs the saved features
     if (smp->n == 0) return 0;
     {
         // the dynamic shared-memory opt-in is a per-DEVICE function attribute: one process may drive several GPUs
@@ -1529,40 +929,18 @@ extern "C" int ngp_net_backward_mlp(const NgpNet* net, const NgpSamples* smp, co
         int dev = 0;
         NGP_CUDA(cudaGetDevice(&dev));
         if (dev < 0 || dev >= 64 || !__atomic_load_n(&attr_set[dev], __ATOMIC_ACQUIRE)) {
-            NGP_CUDA(cudaFuncSetAttribute(k_ngp_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BwdSmem)));
-            NGP_CUDA(cudaFuncSetAttribute(k_ngp_bwd2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Bwd2Smem)));
-            NGP_CUDA(cudaFuncSetAttribute(k_ngp_bwd3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Bwd3Smem) + 128));
+            NGP_CUDA(cudaFuncSetAttribute(k_ngp_bwd3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Bwd3Smem) + 128));
+            NGP_CUDA(cudaFuncSetAttribute(k_ngp_bwd3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Bwd3Smem) + 128));
             if (dev >= 0 && dev < 64) __atomic_store_n(&attr_set[dev], 1, __ATOMIC_RELEASE);
         }
     }
-    static int variant = -1;  // NGP_BWD_VARIANT (env, read once): 2 = wgmma weight gradients (default), 1 = k_ngp_bwd2, 0 = k_ngp_bwd
-    if (variant < 0) {
-        const char* e = getenv("NGP_BWD_VARIANT");
-        variant = e ? atoi(e) : 2;
-    }
     const int64_t n_mtiles = (smp->n + 15) / 16;
-    if (smp->live_idx && (!smp->n_live_dev || variant == 0 || !feat_save)) return NGP_EINVAL;  // live list: k_ngp_bwd2/3 only
-    if (variant == 0 || !feat_save) {
-        const int64_t n_blks = (n_mtiles + BWD_WARPS - 1) / BWD_WARPS;
-        const int grid = (int)(n_blks < (int64_t)ngp_sm_count() ? n_blks : ngp_sm_count());
-        k_ngp_bwd<<<grid, BWD_THREADS, sizeof(BwdSmem), (cudaStream_t)stream>>>(
-            *net, *smp, dL_dsigmas, dL_drgbs, (const uint4*)feat_save, loss_scale, grad_enc, grad_rgb, (uint32_t*)workspace,
-            n_mtiles * 16);
-    } else if (variant == 1) {
-        const int64_t n_blks = (n_mtiles + B2_WARPS - 1) / B2_WARPS;
-        const int grid = (int)(n_blks < (int64_t)ngp_sm_count() ? n_blks : ngp_sm_count());
-        int* sched = sched_slot((cudaStream_t)stream);
-        k_ngp_bwd2<<<grid, B2_THREADS, sizeof(Bwd2Smem), (cudaStream_t)stream>>>(
-            *net, *smp, dL_dsigmas, dL_drgbs, (const uint4*)feat_save, loss_scale, grad_enc, grad_rgb, (uint32_t*)workspace,
-            n_mtiles * 16, sched);
-    } else {
-        const int64_t n_blks = (n_mtiles + B3_WARPS - 1) / B3_WARPS;
-        const int grid = (int)(n_blks < (int64_t)ngp_sm_count() ? n_blks : ngp_sm_count());
-        int* sched = sched_slot((cudaStream_t)stream);
-        k_ngp_bwd3<<<grid, B3_THREADS, sizeof(Bwd3Smem) + 128, (cudaStream_t)stream>>>(
-            *net, *smp, dL_dsigmas, dL_drgbs, (const uint4*)feat_save, loss_scale, grad_enc, grad_rgb, (uint32_t*)workspace,
-            n_mtiles * 16, sched);
-    }
+    const int64_t n_blks = (n_mtiles + B3_WARPS - 1) / B3_WARPS;
+    const int grid = (int)(n_blks < (int64_t)ngp_sm_count() ? n_blks : ngp_sm_count());
+    auto* kernel = feat_save ? k_ngp_bwd3<false> : k_ngp_bwd3<true>;
+    kernel<<<grid, B3_THREADS, sizeof(Bwd3Smem) + 128, (cudaStream_t)stream>>>(
+        *net, *smp, dL_dsigmas, dL_drgbs, (const uint4*)feat_save, loss_scale, grad_enc, grad_rgb, (uint32_t*)workspace,
+        n_mtiles * 16, sched_slot((cudaStream_t)stream));
     NGP_CHECK_LAUNCH();
     NGP_TRACE(6, (cudaStream_t)stream);
     return 0;

@@ -290,7 +290,7 @@ __global__ void k_train_grad_scale(float* __restrict__ scalars, int* __restrict_
 // depends on that ray's composited colour / opacity only): k_train_composite_fw + k_nerf_loss_grad + k_train_composite_bw
 // without the two extra launches and with the second sweep over the ray's samples hitting L1/L2.
 #define CL_WARPS 8  // rays per block of k_train_composite_loss
-// CL_CACHE (template parameter): trips (of 32 samples) of a ray held in registers between the forward and the backward sweep
+#define CL_CACHE 4  // trips (of 32 samples) of a ray held in registers between the forward and the backward sweep (64 regs)
 struct CLSample {
     float sg, de, ti;
     float3 c;
@@ -304,7 +304,6 @@ __device__ __forceinline__ CLSample cl_load(const float* __restrict__ sg, const 
     x.c = make_float3(__ldg(cl + 3 * i), __ldg(cl + 3 * i + 1), __ldg(cl + 3 * i + 2));
     return x;
 }
-template <int CL_CACHE>
 __global__ void __launch_bounds__(CL_WARPS * 32) k_train_composite_loss(const NgpTrainCfg cfg, const int* __restrict__ n_samples, const int* __restrict__ offsets,
                                        const float* __restrict__ sigmas, const float* __restrict__ rgbs,
                                        const float* __restrict__ deltas, const float* __restrict__ ts,
@@ -511,20 +510,9 @@ extern "C" int ngp_render_train_step(const NgpNet* net, const NgpTrainCfg* cfg, 
     NGP_TRACE(13, st);
     rc = ngp_net_forward(net, &smp, 1, b->sigmas, b->rgbs, nullptr, b->feat_save, stream);
     if (rc) return rc;
-    // NGP_CL_CACHE (env, read once): samples/32 of a ray kept in registers by the fused compositing kernel
-    static int cl_cache = -1;
-    if (cl_cache < 0) {
-        const char* e = getenv("NGP_CL_CACHE");
-        cl_cache = e ? atoi(e) : 4;  // 128 samples of a ray in registers (64 regs)
-    }
-#define NGP_LAUNCH_CL(C)                                                                                                   \
-    k_train_composite_loss<C><<<ngp_div_up(n, CL_WARPS), CL_WARPS * 32, 0, st>>>(                                          \
-        *cfg, b->n_samples, b->offsets, b->sigmas, b->rgbs, b->deltas, b->ts, rgb_gt, b->rgb, b->opacity, b->depth, b->dsigmas, \
-        b->drgbs, b->scalars, b->live_idx, b->counters, b->bg_dev)
-    if (cl_cache <= 2) NGP_LAUNCH_CL(2);
-    else if (cl_cache <= 4) NGP_LAUNCH_CL(4);
-    else NGP_LAUNCH_CL(8);
-#undef NGP_LAUNCH_CL
+    k_train_composite_loss<<<ngp_div_up(n, CL_WARPS), CL_WARPS * 32, 0, st>>>(
+        *cfg, b->n_samples, b->offsets, b->sigmas, b->rgbs, b->deltas, b->ts, rgb_gt, b->rgb, b->opacity, b->depth, b->dsigmas,
+        b->drgbs, b->scalars, b->live_idx, b->counters, b->bg_dev);
     NGP_CHECK_LAUNCH();
     NGP_TRACE(4, st);
     k_train_grad_scale<<<1, 1, 0, st>>>(b->scalars, b->counters, 1);

@@ -3,7 +3,7 @@
 Nothing under ngp_pl_b200/ imports this. It is plain torch (any device), so the GPU tests run it on CUDA at training
 sizes and the CPU suite checks it against oracle.torch_ngp_forward / torch_grid_encode on small inputs.
 
-mlp_backward() restates k_ngp_bwd3 (and k_ngp_bwd) at the kernels' own fp16 rounding points:
+mlp_backward() restates k_ngp_bwd3 at the kernel's own fp16 rounding points:
   forward, from the fp16 features:  hid = fp16(relu(feat W1d^T)),  h = fp16(hid W2d^T),  rin = [fp16(SH(d)) | h],
                                     r1 = fp16(relu(rin W1r^T)),  r2 = fp16(relu(r1 W2r^T)),  o = fp16(sigmoid(r2 W3r^T))
   out-gradient chain (scaled by the power-of-two loss scale, each step rounded to fp16):

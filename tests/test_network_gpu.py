@@ -126,9 +126,11 @@ def test_backward_vs_oracle_autograd(oracle):
 
 
 def test_backward_recompute_matches_saved_features():
-    """ngp_net_backward with feat_save == NULL (re-gather) must equal the saved-feature path."""
+    """ngp_net_backward with feat_save == NULL (re-gather) equals the saved-feature path: the feature gradients bit for
+    bit, the weight and table gradients up to the order of their fp32 reductions."""
     from ngp_pl_b200 import _lib
     from ngp_pl_b200.models import networks as N
+    from oracle import grad64
     model = build_model(scale=0.5)
     n = 1000
     x, d = sample_points(n, 0.5, 5)
@@ -143,17 +145,36 @@ def test_backward_recompute_matches_saved_features():
     _lib.check(L.ngp_net_forward(C.byref(net), C.byref(smp), 1, sig.data_ptr(), rgb.data_ptr(), None, feat.data_ptr(), st), "fwd")
     dsig = torch.randn(n, device="cuda") * 1e-3
     drgb = torch.randn(n, 3, device="cuda") * 1e-2
+    n_levels, stride = model.xyz_encoder.n_levels, (n + 15) // 16 * 16
     outs = []
-    ws = torch.empty(L.ngp_net_backward_workspace(n), device="cuda", dtype=torch.uint8)
     for fs in (feat.data_ptr(), None):
         ge = torch.zeros_like(model.xyz_encoder.params)
         gr = torch.zeros_like(model.rgb_net.params)
+        ws = torch.empty(L.ngp_net_backward_workspace(n), device="cuda", dtype=torch.uint8)
         _lib.check(L.ngp_net_backward(C.byref(net), C.byref(smp), dsig.data_ptr(), drgb.data_ptr(), fs, None,
                                       ge.data_ptr(), gr.data_ptr(), ws.data_ptr(), ws.numel(), st), "bwd")
-        outs.append((ge, gr))
+        # the workspace rows the backward writes: one half2 per (level, sample)
+        outs.append((ge, gr, ws.view(torch.int32)[:n_levels * stride].view(n_levels, stride)[:, :n]))
     torch.cuda.synchronize()
-    for a, b in zip(outs[0], outs[1]):
+    (ge_s, gr_s, ws_s), (ge_r, gr_r, ws_r) = outs
+    assert torch.equal(ws_r, ws_s)
+    for a, b in ((ge_s, ge_r), (gr_s, gr_r)):
         assert torch.allclose(a, b, rtol=1e-3, atol=1e-6 + 1e-3 * a.abs().max().item())
+    # the same per-block products in both launches; only the order of the fp32 sums differs: a block's 12 k-steps, the
+    # blocks a CTA takes and <= one reduction per block into dW, each a rounding of at most 2^-24 of sum |terms| = A
+    f16 = lambda t: t if t.dtype == torch.float16 else t.view(torch.float16)
+    ref = grad64.mlp_backward(grad64.decode_feat_save(feat, n), grad64.sh4_64(d), f16(keep[0])[:3072], f16(keep[1]),
+                              dsig, drgb, 1.0, 1)
+    n_add = 13 * ((n + 191) // 192)
+    got_s, got_r = grad64.split_dW(ge_s.double(), gr_s.double()), grad64.split_dW(ge_r.double(), gr_r.double())
+    for k, (_, A, _) in ref["dW"].items():
+        assert ((got_s[k] - got_r[k]).abs() <= 2 * n_add * 2.0 ** -24 * A).all(), k
+    # the table: identical contributions, reduced in another order (m_e + 2 roundings of sum |contrib_e| each)
+    dfeat = ws_s.contiguous().view(torch.float16).view(n_levels, n, 2).permute(1, 0, 2).reshape(n, 2 * n_levels)
+    enc = model.xyz_encoder
+    _, Sabs, m = grad64.grid_scatter(enc.meta, x + 0.5, dfeat, 1.0, enc.n_entries)
+    tol = 2 * (m[:, None] + 2) * 2.0 ** -24 * Sabs
+    assert ((ge_s[3072:].view(-1, 2).double() - ge_r[3072:].view(-1, 2).double()).abs() <= tol).all()
 
 
 def test_loss_scale_invariance():

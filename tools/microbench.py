@@ -65,8 +65,7 @@ def main():
     out["net_fwd_ms"] = timeit(lambda: L.ngp_net_forward(C.byref(net), C.byref(smp), 1, sig.data_ptr(), rgb.data_ptr(), None, feat.data_ptr(), st), flush=flush)
     out["net_fwd_nosave_ms"] = timeit(lambda: L.ngp_net_forward(C.byref(net), C.byref(smp), 1, sig.data_ptr(), rgb.data_ptr(), None, None, st), flush=flush)
     if "--fwd-only" in sys.argv:
-        print(json.dumps({"variant": os.environ.get("NGP_FWD_VARIANT", "default"), "samples": n, "net_fwd_ms": out["net_fwd_ms"],
-                          "net_fwd_nosave_ms": out["net_fwd_nosave_ms"]}))
+        print(json.dumps({"samples": n, "net_fwd_ms": out["net_fwd_ms"], "net_fwd_nosave_ms": out["net_fwd_nosave_ms"]}))
         return
     out["net_density_ms"] = timeit(lambda: L.ngp_net_forward(C.byref(net), C.byref(smp), 0, sig.data_ptr(), None, None, None, st), flush=flush)
     dsig = torch.randn(n, device=dev) * 1e-3; drgb = torch.randn(n, 3, device=dev) * 1e-2

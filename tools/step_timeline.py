@@ -19,7 +19,7 @@ from ngp_pl_b200.models.networks import NGP  # noqa: E402
 from ngp_pl_b200.trainer import Trainer  # noqa: E402
 
 NAMES = {1: "k_sample_rays", 2: "k_train_march", 3: "k_ngp_fwd", 4: "k_train_composite_loss", 5: "k_train_grad_scale",
-         6: "k_ngp_bwd", 7: "k_grid_scatter_merged", 8: "k_adam", 11: "<prepare graph starts>", 13: "<compute graph starts>",
+         6: "k_ngp_bwd3", 7: "k_grid_scatter_merged", 8: "k_adam", 11: "<prepare graph starts>", 13: "<compute graph starts>",
          18: "<update graph starts>", 20: "refresh: memsets", 21: "refresh: k_grid_flags + cub select", 22: "refresh: k_grid_pick",
          30: "  exchange: block 0 enters", 31: "  exchange: start barrier passed (every rank's gradients are complete)",
          32: "  exchange: last block done (reduce-scatter + Adam + all-gather issued)", 33: "  exchange: end barrier passed",
