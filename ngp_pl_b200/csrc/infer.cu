@@ -126,10 +126,9 @@ k_infer_march(const NgpInferCfg cfg, const float* __restrict__ rays_o, const flo
                 t = t_cur[r];
                 const float t2 = t_end[r];
                 float dt;
-                uint32_t cache_idx = 0xffffffffu;
-                bool cache_occ = false;
+                MarchCache cache;
                 while (t < t2 && n < S) {
-                    if (march_visit_cached<CONST_DT, ONE_CASCADE>(ray, c, t, dt, cache_idx, cache_occ)) {
+                    if (march_visit_t<CONST_DT, ONE_CASCADE>(ray, c, t, dt, &cache)) {
                         my[n] = make_float2(t, dt);
                         t = __fadd_rn(t, dt);
                         ++n;
@@ -382,17 +381,12 @@ static int infer_round(const NgpNet* net, const NgpInferCfg* cfg, const InferWs&
     const int grid_m = (int)min((int64_t)ngp_div_up(n, INFER_THREADS), (int64_t)sms * 16);
     const int grid_c = (int)min((int64_t)ngp_div_up(n, 128), (int64_t)sms * 16);
     // the test-time step bounds use `cascades` where the train kernel uses `scale` (reference raymarching.cu:370,399)
-    const bool const_dt = cfg->exp_step_factor == 0.0f &&
-                          1.73205080757f / (float)cfg->max_samples <= (float)cfg->cascades * 3.46410161514f / (float)cfg->grid_size;
-#define NGP_LAUNCH_IM(CD, OC)                                                                                              \
-    k_infer_march<CD, OC><<<grid_m, INFER_THREADS, 0, st>>>(*cfg, rays_o, rays_d, density_bitfield, W.t_cur, W.t_end,      \
-                                                            W.alive[cur], W.alive_cnt + cur, W.ray_start, W.ray_n, W.ray_idx, \
-                                                            W.ts, W.deltas, W.state)
-    if (const_dt && cfg->cascades == 1) NGP_LAUNCH_IM(true, true);
-    else if (const_dt) NGP_LAUNCH_IM(true, false);
-    else if (cfg->cascades == 1) NGP_LAUNCH_IM(false, true);
-    else NGP_LAUNCH_IM(false, false);
-#undef NGP_LAUNCH_IM
+    const bool const_dt = march_const_dt(cfg->exp_step_factor, cfg->max_samples, (float)cfg->cascades, cfg->grid_size);
+    march_dispatch(const_dt, cfg->cascades, [&](auto cd, auto oc) {
+        k_infer_march<decltype(cd)::value, decltype(oc)::value><<<grid_m, INFER_THREADS, 0, st>>>(
+            *cfg, rays_o, rays_d, density_bitfield, W.t_cur, W.t_end, W.alive[cur], W.alive_cnt + cur, W.ray_start, W.ray_n,
+            W.ray_idx, W.ts, W.deltas, W.state);
+    });
     NGP_CHECK_LAUNCH();
     NgpSamples smp;
     smp.xyzs = nullptr; smp.dirs = nullptr; smp.rays_o = rays_o; smp.rays_d = rays_d; smp.ray_idx = W.ray_idx; smp.ts = W.ts;

@@ -1,4 +1,5 @@
-// Occupancy-grid ray marcher core (device functions shared by every kernel that marches).
+// Occupancy-grid ray marcher core: the device functions shared by every kernel that marches, and the host-side
+// choice of which specialisation to launch.
 //
 // Parity contract: the per-ray sequence of (t, dt, xyz) must be BIT-EXACT with the reference's
 // raymarching_train_kernel / raymarching_test_kernel (reference models/csrc/raymarching.cu:166-280,
@@ -7,6 +8,7 @@
 // step is spelled with an explicit intrinsic (__fmaf_rn / __fmul_rn / __fadd_rn / __fdiv_rn), so the
 // result does not depend on how the compiler chooses to contract the surrounding code.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 
 struct MarchConst {
@@ -101,56 +103,6 @@ __device__ __forceinline__ float2 ray_aabb(const MarchRay& r, float cx, float cy
     return make_float2(t1, t2);
 }
 
-// One visit of the marcher at parameter t. Returns true when the cell under the ray is occupied
-// (then (x,y,z,dt) describe the sample and the caller advances t += dt); otherwise t has already
-// been advanced past the empty cell.
-__device__ __forceinline__ bool march_visit(const MarchRay& r, const MarchConst& c, float& t,
-                                            float& x, float& y, float& z, float& dt) {
-    x = __fmaf_rn(r.dx, t, r.ox);
-    y = __fmaf_rn(r.dy, t, r.oy);
-    z = __fmaf_rn(r.dz, t, r.oz);
-    dt = march_dt(t, c);
-
-    int e_pos, e_dt;
-    frexpf(fmaxf(fabsf(x), fmaxf(fabsf(y), fabsf(z))), &e_pos);
-    frexpf(__fmul_rn(dt, c.gs_f), &e_dt);
-    const int mip_pos = min(c.cascades - 1, max(0, e_pos + 1));
-    const int mip_dt = min(c.cascades - 1, max(0, e_dt));
-    const int mip = max(mip_pos, mip_dt);
-
-    const float mip_bound = fminf(scalbnf(1.0f, mip - 1), c.scale);
-    const float mip_bound_inv = __fdiv_rn(1.0f, mip_bound);
-
-    float vx = __fmul_rn(__fmul_rn(__fmaf_rn(x, mip_bound_inv, 1.0f), 0.5f), c.gs_f);
-    float vy = __fmul_rn(__fmul_rn(__fmaf_rn(y, mip_bound_inv, 1.0f), 0.5f), c.gs_f);
-    float vz = __fmul_rn(__fmul_rn(__fmaf_rn(z, mip_bound_inv, 1.0f), 0.5f), c.gs_f);
-    const int nx = (int)fmaxf(0.0f, fminf(vx, c.gs_m1));
-    const int ny = (int)fmaxf(0.0f, fminf(vy, c.gs_m1));
-    const int nz = (int)fmaxf(0.0f, fminf(vz, c.gs_m1));
-
-    const uint32_t idx = (uint32_t)mip * c.grid_size3 + morton_encode3((uint32_t)nx, (uint32_t)ny, (uint32_t)nz);
-    const bool occ = (__ldg(c.bitfield + (idx >> 3)) >> (idx & 7u)) & 1u;
-    if (occ) return true;
-
-    // distance to the exit face of this cell along each axis, then step-quantised advance
-    float a;
-    a = __fmaf_rn(r.sx, 0.5f, __fadd_rn((float)nx, 0.5f));
-    a = __fmaf_rn(__fmul_rn(a, c.gs_inv), 2.0f, -1.0f);
-    const float tx = __fmul_rn(__fmaf_rn(mip_bound, a, -x), r.ix);
-    a = __fmaf_rn(r.sy, 0.5f, __fadd_rn((float)ny, 0.5f));
-    a = __fmaf_rn(__fmul_rn(a, c.gs_inv), 2.0f, -1.0f);
-    const float ty = __fmul_rn(__fmaf_rn(mip_bound, a, -y), r.iy);
-    a = __fmaf_rn(r.sz, 0.5f, __fadd_rn((float)nz, 0.5f));
-    a = __fmaf_rn(__fmul_rn(a, c.gs_inv), 2.0f, -1.0f);
-    const float tz = __fmul_rn(__fmaf_rn(mip_bound, a, -z), r.iz);
-
-    const float t_target = __fadd_rn(t, fmaxf(0.0f, fminf(tx, fminf(ty, tz))));
-    do {
-        t = __fadd_rn(t, march_dt(t, c));
-    } while (t < t_target);
-    return false;
-}
-
 // Train-time start jitter (reference raymarching.cu:195-198): only for rays that hit the box.
 __device__ __forceinline__ float march_jitter(float t1, float noise, const MarchConst& c) {
     if (t1 >= 0.0f) t1 = __fmaf_rn(march_dt(t1, c), noise, t1);
@@ -158,18 +110,8 @@ __device__ __forceinline__ float march_jitter(float t1, float noise, const March
 }
 
 // -------------------------------------------------------------------------------------------------
-// Warp-cooperative marcher (one WARP per ray), bit-exact with the serial one.
-//
-// Every parameter value the reference ever visits lies on the ray's STEP CHAIN
-//     c_0 = t_start,   c_{k+1} = c_k (+) dt(c_k)          ((+) = one fp32 rounded add)
-// because both branches of its loop advance t the same way: an occupied visit does t += dt(t), an empty
-// visit repeats t += dt(t) until t >= t_target. So the marcher is a walk over that chain: at a visited
-// point test the cell; if occupied emit it and go to the next chain point, else jump to the first chain
-// point >= t_target. Here a warp materialises 32 consecutive chain points (31 dependent rounded adds,
-// identical roundings to the serial code), tests all 32 cells at once, and resolves which of them the
-// serial walk would have visited with ballots. One thread per ray is latency bound (a dependent
-// load + ~60 dependent ALU ops per visit, ~2 warps per SM at 8192 rays); this keeps the same
-// sequence of fp32 operations per chain point but runs 32 of them side by side.
+// One visit of the marcher at parameter t: the only place the per-point arithmetic is written. The serial
+// visit below and the warp marcher (which probes 32 chain points at once) both use march_probe.
 // -------------------------------------------------------------------------------------------------
 struct MarchProbe {
     bool occ;
@@ -177,10 +119,20 @@ struct MarchProbe {
     float t_target;  // where an empty visit here jumps to (valid when !occ)
 };
 
+// One-entry cache of the occupancy lookup for a thread that marches one ray serially: consecutive samples of a ray fall
+// into the same cell of the 128^3 grid ~4.6 times in a row (step 1/590 of the box diagonal vs cell 1/128), and the bit
+// load is the one dependent global load on the visit's critical path. idx = 0xffffffff: empty.
+struct MarchCache {
+    uint32_t idx = 0xffffffffu;
+    bool occ = false;
+};
+
 // ONE_CASCADE: with a single cascade both mip_from_pos and mip_from_dt clamp to 0 (min(cascades-1, .)), so
 // mip = 0 and mip_bound = min(2^-1, scale) for every sample: the two frexpf, the scalbnf and the division drop out.
+// With a cache the bit lookup is reused while the cell index is unchanged (same arithmetic, same roundings).
 template <bool ONE_CASCADE>
-__device__ __forceinline__ MarchProbe march_probe(const MarchRay& r, const MarchConst& c, float t) {
+__device__ __forceinline__ MarchProbe march_probe(const MarchRay& r, const MarchConst& c, float t,
+                                                  MarchCache* cache = nullptr) {
     MarchProbe o;
     const float x = __fmaf_rn(r.dx, t, r.ox);
     const float y = __fmaf_rn(r.dy, t, r.oy);
@@ -206,7 +158,16 @@ __device__ __forceinline__ MarchProbe march_probe(const MarchRay& r, const March
     const int ny = (int)fmaxf(0.0f, fminf(vy, c.gs_m1));
     const int nz = (int)fmaxf(0.0f, fminf(vz, c.gs_m1));
     const uint32_t idx = (uint32_t)mip * c.grid_size3 + morton_encode3((uint32_t)nx, (uint32_t)ny, (uint32_t)nz);
-    o.occ = (__ldg(c.bitfield + (idx >> 3)) >> (idx & 7u)) & 1u;
+    if (!cache) {
+        o.occ = (__ldg(c.bitfield + (idx >> 3)) >> (idx & 7u)) & 1u;
+    } else {
+        if (idx != cache->idx) {
+            cache->occ = (__ldg(c.bitfield + (idx >> 3)) >> (idx & 7u)) & 1u;
+            cache->idx = idx;
+        }
+        o.occ = cache->occ;
+    }
+    // distance to the exit face of this cell along each axis
     float a;
     a = __fmaf_rn(r.sx, 0.5f, __fadd_rn((float)nx, 0.5f));
     a = __fmaf_rn(__fmul_rn(a, c.gs_inv), 2.0f, -1.0f);
@@ -221,11 +182,14 @@ __device__ __forceinline__ MarchProbe march_probe(const MarchRay& r, const March
     return o;
 }
 
-// Serial visit with the specialisations of march_probe (ONE_CASCADE drops the two frexpf, the scalbnf and the division;
-// CONST_DT the multiply / clamp of the step): same values, same roundings as march_visit().
+// Serial visit. Returns true when the cell under the ray is occupied (then dt is the sample's step, the sample sits at
+// fma(d, t, o) and the caller advances t += dt); otherwise t has already been advanced past the empty cell, step by step
+// like the reference. CONST_DT: the step is the constant dt_lo (see march_const_dt), the same value without the
+// multiply and clamp.
 template <bool CONST_DT, bool ONE_CASCADE>
-__device__ __forceinline__ bool march_visit_t(const MarchRay& r, const MarchConst& c, float& t, float& dt) {
-    const MarchProbe pr = march_probe<ONE_CASCADE>(r, c, t);
+__device__ __forceinline__ bool march_visit_t(const MarchRay& r, const MarchConst& c, float& t, float& dt,
+                                              MarchCache* cache = nullptr) {
+    const MarchProbe pr = march_probe<ONE_CASCADE>(r, c, t, cache);
     dt = pr.dt;
     if (pr.occ) return true;
     do {
@@ -234,58 +198,20 @@ __device__ __forceinline__ bool march_visit_t(const MarchRay& r, const MarchCons
     return false;
 }
 
-// The same visit with a one-entry cache of the occupancy lookup: consecutive samples of a ray fall into the same cell of
-// the 128^3 grid ~4.6 times in a row (step 1/590 of the box diagonal vs cell 1/128), and the bit load is the one dependent
-// global load on the visit's critical path. (cache_idx = 0xffffffff: empty.) Same arithmetic, same roundings.
-template <bool CONST_DT, bool ONE_CASCADE>
-__device__ __forceinline__ bool march_visit_cached(const MarchRay& r, const MarchConst& c, float& t, float& dt,
-                                                   uint32_t& cache_idx, bool& cache_occ) {
-    const float x = __fmaf_rn(r.dx, t, r.ox);
-    const float y = __fmaf_rn(r.dy, t, r.oy);
-    const float z = __fmaf_rn(r.dz, t, r.oz);
-    dt = march_dt(t, c);
-    int mip = 0;
-    float mip_bound, mip_bound_inv;
-    if (ONE_CASCADE) {
-        mip_bound = c.mb0;
-        mip_bound_inv = c.mb0_inv;
-    } else {
-        int e_pos, e_dt;
-        frexpf(fmaxf(fabsf(x), fmaxf(fabsf(y), fabsf(z))), &e_pos);
-        frexpf(__fmul_rn(dt, c.gs_f), &e_dt);
-        mip = max(min(c.cascades - 1, max(0, e_pos + 1)), min(c.cascades - 1, max(0, e_dt)));
-        mip_bound = fminf(scalbnf(1.0f, mip - 1), c.scale);
-        mip_bound_inv = __fdiv_rn(1.0f, mip_bound);
-    }
-    const float vx = __fmul_rn(__fmul_rn(__fmaf_rn(x, mip_bound_inv, 1.0f), 0.5f), c.gs_f);
-    const float vy = __fmul_rn(__fmul_rn(__fmaf_rn(y, mip_bound_inv, 1.0f), 0.5f), c.gs_f);
-    const float vz = __fmul_rn(__fmul_rn(__fmaf_rn(z, mip_bound_inv, 1.0f), 0.5f), c.gs_f);
-    const int nx = (int)fmaxf(0.0f, fminf(vx, c.gs_m1));
-    const int ny = (int)fmaxf(0.0f, fminf(vy, c.gs_m1));
-    const int nz = (int)fmaxf(0.0f, fminf(vz, c.gs_m1));
-    const uint32_t idx = (uint32_t)mip * c.grid_size3 + morton_encode3((uint32_t)nx, (uint32_t)ny, (uint32_t)nz);
-    if (idx != cache_idx) {
-        cache_occ = (__ldg(c.bitfield + (idx >> 3)) >> (idx & 7u)) & 1u;
-        cache_idx = idx;
-    }
-    if (cache_occ) return true;
-    float a;
-    a = __fmaf_rn(r.sx, 0.5f, __fadd_rn((float)nx, 0.5f));
-    a = __fmaf_rn(__fmul_rn(a, c.gs_inv), 2.0f, -1.0f);
-    const float tx = __fmul_rn(__fmaf_rn(mip_bound, a, -x), r.ix);
-    a = __fmaf_rn(r.sy, 0.5f, __fadd_rn((float)ny, 0.5f));
-    a = __fmaf_rn(__fmul_rn(a, c.gs_inv), 2.0f, -1.0f);
-    const float ty = __fmul_rn(__fmaf_rn(mip_bound, a, -y), r.iy);
-    a = __fmaf_rn(r.sz, 0.5f, __fadd_rn((float)nz, 0.5f));
-    a = __fmaf_rn(__fmul_rn(a, c.gs_inv), 2.0f, -1.0f);
-    const float tz = __fmul_rn(__fmaf_rn(mip_bound, a, -z), r.iz);
-    const float t_target = __fadd_rn(t, fmaxf(0.0f, fminf(tx, fminf(ty, tz))));
-    do {
-        t = __fadd_rn(t, CONST_DT ? c.dt_lo : march_dt(t, c));
-    } while (t < t_target);
-    return false;
-}
-
+// -------------------------------------------------------------------------------------------------
+// Warp-cooperative marcher (one WARP per ray), bit-exact with the serial one.
+//
+// Every parameter value the reference ever visits lies on the ray's STEP CHAIN
+//     c_0 = t_start,   c_{k+1} = c_k (+) dt(c_k)          ((+) = one fp32 rounded add)
+// because both branches of its loop advance t the same way: an occupied visit does t += dt(t), an empty
+// visit repeats t += dt(t) until t >= t_target. So the marcher is a walk over that chain: at a visited
+// point test the cell; if occupied emit it and go to the next chain point, else jump to the first chain
+// point >= t_target. Here a warp materialises 32 consecutive chain points (31 dependent rounded adds,
+// identical roundings to the serial code), tests all 32 cells at once, and resolves which of them the
+// serial walk would have visited with ballots. One thread per ray is latency bound (a dependent
+// load + ~60 dependent ALU ops per visit, ~2 warps per SM at 8192 rays); this keeps the same
+// sequence of fp32 operations per chain point but runs 32 of them side by side.
+// -------------------------------------------------------------------------------------------------
 // March one ray with a full warp. emit(k, t, dt) is called by the lane owning the k-th sample
 // (k = 0.. in ray order). Returns the number of samples (same in every lane) and leaves in t_resume the
 // chain point the serial marcher would visit next (what raymarching_test stores back into hits_t).
@@ -427,4 +353,25 @@ __device__ __forceinline__ int march_ray_warp(const MarchRay& ray, const MarchCo
     }
     if (t_resume) *t_resume = resume;
     return n;
+}
+
+// -------------------------------------------------------------------------------------------------
+// Host side: which specialisation of a marching kernel to launch.
+// -------------------------------------------------------------------------------------------------
+// The step is the constant dt_lo when exp_step_factor == 0 and dt_lo <= dt_hi: march_dt clamps t*0 up to dt_lo for every
+// finite t >= 0. dt_scale is what make_march_const receives for dt_hi (the train kernel's scale, the test kernel's cascades).
+inline bool march_const_dt(float esf, int max_samples, float dt_scale, int grid_size) {
+    return esf == 0.0f && 1.73205080757f / (float)max_samples <= dt_scale * 3.46410161514f / (float)grid_size;
+}
+
+// Calls launch(std::integral_constant<bool, CONST_DT>{}, std::integral_constant<bool, ONE_CASCADE>{}) for the instance
+// that serves (const_dt, cascades); the call site launches k<decltype(cd)::value, decltype(oc)::value>.
+template <class Launch>
+inline void march_dispatch(bool const_dt, int cascades, Launch&& launch) {
+    using T = std::true_type;
+    using F = std::false_type;
+    if (const_dt && cascades == 1) launch(T{}, T{});
+    else if (const_dt) launch(T{}, F{});
+    else if (cascades == 1) launch(F{}, T{});
+    else launch(F{}, F{});
 }

@@ -10,8 +10,6 @@
 #include <cub/device/device_select.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
 
-static inline int one_thread_per_ray_block(int n_rays) { return n_rays >= ngp_sm_count() * 128 * 4 ? 128 : 32; }
-
 // -------------------------------------------------------------------------------------------------
 // 1. AABB + near clamp + jittered march, ONE pass: samples go to a per-ray staging row
 //    (reference intersection.cu:25-56, rendering.py:29, raymarching.cu:166-235)
@@ -154,22 +152,16 @@ extern "C" int ngp_render_train_march(const NgpTrainCfg* cfg, const NgpTrainBuff
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int n = cfg->n_rays;
-    // exp_step_factor == 0 with dt_lo <= dt_hi: every step equals dt_lo (clamp(0, lo, hi))
-    const bool const_dt = cfg->exp_step_factor == 0.0f &&
-                          1.73205080757f / (float)cfg->max_samples <= cfg->scale * 3.46410161514f / (float)cfg->grid_size;
+    const bool const_dt = march_const_dt(cfg->exp_step_factor, cfg->max_samples, cfg->scale, cfg->grid_size);
     const dim3 mg(ngp_div_up((int64_t)n * 32, 128));
     // accumulators of the march kernel's segment allocation: two ints at the head of scan_temp, zero between launches
     // (zeroed once by the caller -- torch allocates scan_temp zero-filled in the Trainer -- and re-armed by the kernel)
     int* acc = (int*)b->scan_temp;
-#define NGP_LAUNCH_MARCH(CD, OC)                                                                                        \
-    k_train_march<CD, OC><<<mg, 128, 0, st>>>(*cfg, b->rays_o, b->rays_d, b->noise, b->density_bitfield, b->stage_t, \
-                                              b->stage_dt, b->n_samples, b->offsets, b->ray_idx, b->ts, b->deltas,    \
-                                              b->counters, acc)
-    if (const_dt && cfg->cascades == 1) NGP_LAUNCH_MARCH(true, true);
-    else if (const_dt) NGP_LAUNCH_MARCH(true, false);
-    else if (cfg->cascades == 1) NGP_LAUNCH_MARCH(false, true);
-    else NGP_LAUNCH_MARCH(false, false);
-#undef NGP_LAUNCH_MARCH
+    march_dispatch(const_dt, cfg->cascades, [&](auto cd, auto oc) {
+        k_train_march<decltype(cd)::value, decltype(oc)::value><<<mg, 128, 0, st>>>(
+            *cfg, b->rays_o, b->rays_d, b->noise, b->density_bitfield, b->stage_t, b->stage_dt, b->n_samples, b->offsets,
+            b->ray_idx, b->ts, b->deltas, b->counters, acc);
+    });
     NGP_CHECK_LAUNCH();
     NGP_TRACE(2, st);
     return 0;

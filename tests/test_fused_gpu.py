@@ -224,16 +224,22 @@ def test_update_density_grid_semantics():
     assert not torch.equal(b2, model.density_grid)
 
 
+def frame_rays(which):
+    """one 160x120 camera view of the synthetic Lego or mip360 scene"""
+    from ngp_pl_b200 import synth
+    K = synth.intrinsics(W=160, H=120, fx=1111.11 / 5)
+    dirs = synth.ray_directions(K, "cuda")
+    pose = torch.as_tensor(synth.camera_poses(3, radius=1.5 if which == "lego" else 0.9)[1]).cuda()
+    return synth.get_rays(dirs, pose)
+
+
 @pytest.mark.parametrize("which", ["lego", "mip360"])
 def test_fused_inference_matches_operator_loop(which):
     from ngp_pl_b200 import synth
     from ngp_pl_b200.models.rendering import render
     scene = synth.lego_scene(0) if which == "lego" else synth.mip360_scene(0)
     model = make_model(scene, amp=0.5)
-    K = synth.intrinsics(W=160, H=120, fx=1111.11 / 5)
-    dirs = synth.ray_directions(K, "cuda")
-    pose = torch.as_tensor(synth.camera_poses(3, radius=1.5 if which == "lego" else 0.9)[1]).cuda()
-    o, d = synth.get_rays(dirs, pose)
+    o, d = frame_rays(which)
     kw = {} if scene.exp_step_factor == 0 else {"exp_step_factor": scene.exp_step_factor}
     a = render(model, o, d, test_time=True, fused=True, **kw)
     b = render(model, o, d, test_time=True, fused=False, **kw)
@@ -244,6 +250,30 @@ def test_fused_inference_matches_operator_loop(which):
     # both evaluate the reference's per-round quota max(min(N_rays // N_alive, 64), min_samples) (rendering.py:80) from the same
     # alive counts, so the marched totals agree up to the rays whose termination round moves with the last bits of sigma
     assert ta > 0 and abs(ta - tb) <= 0.01 * tb
+
+
+@pytest.mark.parametrize("esf", [0.0, 1.0 / 256])
+@pytest.mark.parametrize("which", ["lego", "mip360"])
+def test_fused_inference_marcher_bitwise_vs_operator_loop(which, esf):
+    """The inference wavefront's marcher (k_infer_march: thread per ray with the cached cell visit, warp per ray in the
+    late rounds) against raymarching_test, bit for bit. With every MLP weight zero, sigma = exp(0) = 1 and
+    rgb = sigmoid(0) = 0.5 exactly in both paths, and both compositing loops do the same serial fp32 operations, so the
+    termination rounds, alive counts and quotas agree and any difference comes from the marchers. bg is 0 or 1, so
+    bg * (1 - opacity) is exact. (lego, mip360) x (esf 0, 1/256) runs all four step-kind x cascade instances."""
+    from ngp_pl_b200 import synth
+    from ngp_pl_b200.models.rendering import render
+    scene = synth.lego_scene(0) if which == "lego" else synth.mip360_scene(0)
+    model = make_model(scene, amp=0.5)
+    with torch.no_grad():
+        model.xyz_encoder.params[:3072] = 0
+        model.rgb_net.params.zero_()
+    o, d = frame_rays(which)
+    a = render(model, o, d, test_time=True, exp_step_factor=esf)
+    b = render(model, o, d, test_time=True, fused=False, exp_step_factor=esf)
+    assert int(a["total_samples"]) == int(b["total_samples"]) > 0
+    for k in ("opacity", "depth", "rgb"):
+        bad = (a[k].view(torch.int32) != b[k].view(torch.int32)).sum().item()
+        assert bad == 0, "%s: %d/%d elements differ bitwise" % (k, bad, a[k].numel())
 
 
 def test_training_converges_and_graph_capture_works():
