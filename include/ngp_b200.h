@@ -413,6 +413,23 @@ int ngp_render_infer_frame(const NgpNet* net, const NgpInferCfg* cfg, const floa
                            const uint8_t* density_bitfield, float* opacity, float* depth, float* rgb, int64_t* total_samples,
                            void* workspace, size_t workspace_bytes, void* stream);
 
+/* ----------------------------------------------------------------------------------------------
+ * Validation metrics of one rendered view (reference train.py:193-237): the per-image PSNR of torchmetrics'
+ * PeakSignalNoiseRatio(data_range=1) / metrics.py:14-15 and SSIM of StructuralSimilarityIndexMeasure(data_range=1)
+ * (11-tap Gaussian window, sigma 1.5, only windows wholly inside the image, variances not clamped).
+ * -------------------------------------------------------------------------------------------- */
+size_t ngp_image_metrics_workspace(int H, int W); /* bytes; the buffer must be ZERO-INITIALISED once by the caller (an
+                                                     arrival counter the kernel re-arms); one launch at a time uses it */
+/* pred: fp32 (H*W,3) in the reference's '(h w) c' pixel order; gt: the same layout, uint8 read as v/255 in fp32
+ * (gt_is_u8 != 0) or fp32. Writes, on the device, *out_sse = sum of squared errors over all 3*H*W values (double; PSNR =
+ * -10 log10(sse / (3*H*W)) for data_range 1) and *out_ssim = the mean SSIM over the window centres [5,H-5) x [5,W-5) and
+ * the three channels (double; c1 = (0.01 data_range)^2, c2 = (0.03 data_range)^2). out_ssim may be NULL: then only the
+ * squared error is computed and any H, W >= 1 will do (a flat list of n pixels is H = 1, W = n). NGP_EINVAL for a NULL
+ * pred, gt, out_sse or workspace, H or W < 11 with out_ssim, data_range <= 0, or a short workspace. One kernel; the
+ * result does not depend on scheduling (per-block partials summed in block order), so two calls are bitwise equal. */
+int ngp_image_metrics(const float* pred, const void* gt, int gt_is_u8, int H, int W, float data_range, double* out_sse,
+                      double* out_ssim, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -159,6 +159,8 @@ SIGNATURES = {
     "ngp_update_density_grid": (_i, [C.POINTER(NgpNet), _P, _P, _P, _i, _i, _f, _f, _i, _f, C.c_uint32, _P, _sz, _P]),
     "ngp_update_density_grid_pick": (_i, [_P, _i, _i, _f, _f, _i, C.c_uint32, _P, _sz, _P]),
     "ngp_update_density_grid_eval": (_i, [C.POINTER(NgpNet), _P, _P, _P, _i, _i, _f, _i, _f, _P, _sz, _P]),
+    "ngp_image_metrics_workspace": (_sz, [_i, _i]),
+    "ngp_image_metrics": (_i, [_P, _P, _i, _i, _i, _f, _P, _P, _P, _sz, _P]),
 }
 
 _lib = None

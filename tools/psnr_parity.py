@@ -2,7 +2,8 @@
 (reference vren kernels + unmodified reference Python + tinycudann stand-in) on the same synthetic Lego scene with the
 reference's recipe -- 8192 rays/step, Adam lr 1e-2 eps 1e-15, CosineAnnealingLR(T_max = epochs, eta_min = lr/30) stepped
 per 1000-step epoch (train.py:131-137), occupancy refresh every 16 steps with a 256-step warm-up -- for the same number
-of steps, and render the same held-out 800x800 views at the same checkpoints.
+of steps, and render the same held-out 800x800 views at the same checkpoints. Both arms are scored by
+ngp_pl_b200.metrics.evaluate (per-view PSNR and SSIM as the reference's validation pass computes them).
 
     python tools/psnr_parity.py [steps] [out.json] [--tcnn fast|standin] [--views 8] [--res 800] [--no-cosine]
 """
@@ -18,6 +19,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ngp_pl_b200 import synth  # noqa: E402
+from ngp_pl_b200.metrics import evaluate  # noqa: E402
 from ngp_pl_b200.models.networks import NGP  # noqa: E402
 from ngp_pl_b200.models.rendering import render  # noqa: E402
 from ngp_pl_b200.trainer import CosineAnnealingLR, Trainer  # noqa: E402
@@ -25,17 +27,17 @@ from ngp_pl_b200.trainer import CosineAnnealingLR, Trainer  # noqa: E402
 N_RAYS = 8192
 
 
-def eval_psnr(render_fn, scene, n_views, res):
+def held_out_views(scene, n_views, res):
     K = synth.intrinsics(W=res, H=res, fx=1111.11 * res / 800)
     dirs = synth.ray_directions(K, "cuda")
     poses = torch.as_tensor(synth.camera_poses(n_views, seed=4321)).cuda()
-    out = []
-    for i in range(n_views):
-        o, d = synth.get_rays(dirs, poses[i])
-        rgb = render_fn(o, d)["rgb"].float()
-        gt = synth.trace(scene, o, d)
-        out.append(-10 * float(torch.log10(((rgb - gt) ** 2).mean())))
-    return float(np.mean(out)), out
+    images = torch.stack([synth.trace(scene, *synth.get_rays(dirs, poses[i])) for i in range(n_views)])
+    return poses, dirs, images
+
+
+def eval_views(render_fn, views, res):
+    poses, dirs, images = views
+    return evaluate(render_fn, poses, dirs, images, (res, res))
 
 
 def checkpoints(steps):
@@ -56,6 +58,7 @@ def main():
     epochs = max(1, steps // 1000)
     scene = synth.lego_scene(0)
     cps = checkpoints(steps)
+    views = held_out_views(scene, a.views, a.res)
     res = {"steps": steps, "rays_per_step": N_RAYS, "views": a.views, "resolution": a.res,
            "lr_schedule": None if a.no_cosine else "CosineAnnealingLR(T_max=%d epochs of 1000 steps, eta_min=lr/30)" % epochs,
            "reference_tcnn": a.tcnn, "checkpoints": cps}
@@ -80,11 +83,13 @@ def main():
             mses.append(tr.scalars[2].item() / (3 * N_RAYS))
         if step in cps:
             torch.cuda.synchronize()
-            p, views = eval_psnr(lambda o, d: render(model, o, d, test_time=True), scene, a.views, a.res)
+            ev = eval_views(lambda o, d: render(model, o, d, test_time=True), views, a.res)
             tp = -10 * math.log10(max(float(np.mean(mses[-50:])), 1e-12))
-            curve[str(step)] = {"test_psnr": p, "views": views, "train_psnr_mean50": tp, "lr": tr.lr,
+            curve[str(step)] = {"test_psnr": ev["psnr"], "test_ssim": ev["ssim"], "views": ev["psnr_per_view"],
+                                "views_ssim": ev["ssim_per_view"], "train_psnr_mean50": tp, "lr": tr.lr,
                                 "samples_per_ray": tr.stats()["rm_samples"] / N_RAYS}
-            print("b200 step %d: test %.3f dB  train(mean of 50 batches) %.3f dB  lr %.2e" % (step, p, tp, tr.lr), flush=True)
+            print("b200 step %d: test %.3f dB  test_ssim %.4f  train(mean of 50 batches) %.3f dB  lr %.2e" % (
+                step, ev["psnr"], ev["ssim"], tp, tr.lr), flush=True)
     res["b200"] = curve
     res["b200_wall_s"] = time.perf_counter() - t0
     del tr
@@ -125,17 +130,20 @@ def main():
                 mses.append(((r["rgb"].float() - rgb) ** 2).mean().item())
             if step in cps:
                 torch.cuda.synchronize()
-                p, views = eval_psnr(ref_render, scene, a.views, a.res)
+                ev = eval_views(ref_render, views, a.res)
                 tp = -10 * math.log10(max(float(np.mean(mses[-50:])), 1e-12))
-                curve[str(step)] = {"test_psnr": p, "views": views, "train_psnr_mean50": tp, "lr": opt.param_groups[0]["lr"],
+                curve[str(step)] = {"test_psnr": ev["psnr"], "test_ssim": ev["ssim"], "views": ev["psnr_per_view"],
+                                    "views_ssim": ev["ssim_per_view"], "train_psnr_mean50": tp, "lr": opt.param_groups[0]["lr"],
                                     "samples_per_ray": float(r["rm_samples"]) / N_RAYS}
-                print("reference step %d: test %.3f dB  train(mean of 50 batches) %.3f dB" % (step, p, tp), flush=True)
+                print("reference step %d: test %.3f dB  test_ssim %.4f  train(mean of 50 batches) %.3f dB" % (
+                    step, ev["psnr"], ev["ssim"], tp), flush=True)
             if sch is not None and step % 1000 == 0:
                 sch.step()  # PL steps the scheduler at the end of every (1000-step) epoch
         res["reference"] = curve
         res["reference_wall_s"] = time.perf_counter() - t0
         res["delta_db"] = {k: res["b200"][k]["test_psnr"] - curve[k]["test_psnr"] for k in curve}
         res["delta_db_final"] = res["delta_db"][str(steps)]
+        res["delta_ssim"] = {k: res["b200"][k]["test_ssim"] - curve[k]["test_ssim"] for k in curve}
         res["delta_train_db"] = {k: res["b200"][k]["train_psnr_mean50"] - curve[k]["train_psnr_mean50"] for k in curve}
     print(json.dumps(res))
     if a.out:
