@@ -430,6 +430,51 @@ size_t ngp_image_metrics_workspace(int H, int W); /* bytes; the buffer must be Z
 int ngp_image_metrics(const float* pred, const void* gt, int gt_is_u8, int H, int W, float data_range, double* out_sse,
                       double* out_ssim, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ----------------------------------------------------------------------------------------------
+ * Mesh extraction of a trained model. Replaces the mesh cell of the reference's test.ipynb, which evaluates
+ * model.density on an N^3 np.meshgrid materialised on the host and runs mcubes.marching_cubes(sigma, 20.) on the CPU.
+ * A lattice has n[a] >= 2 points on axis a; point (i, j, k) lies at x_a = lo[a] + (float)idx_a * step[a] (an fp32
+ * multiply, then an fp32 add; axis 0 is x) and has linear index (i*n1 + j)*n2 + k.
+ * -------------------------------------------------------------------------------------------- */
+typedef struct {
+    int32_t n[3];
+    float lo[3];
+    float step[3]; /* (hi - lo) / (n - 1) in fp32 */
+} NgpLattice;
+
+/* sigma (n0*n1*n2 fp32, linear-index order) = NGP.density at every lattice point: bitwise what ngp_net_forward(want_rgb
+ * = 0) gives for the same points materialised as xyzs. The points are computed in the kernel, never stored. Points
+ * outside the model's box are allowed (the encoding treats them as ngp_net_forward does). */
+int ngp_density_lattice(const NgpNet* net, const NgpLattice* lat, float* sigma, void* stream);
+
+/* Marching cubes on a volume (n0*n1*n2 fp32 in linear-index order) at level `iso`:
+ *   - a lattice value is inside iff v > iso (NaN is outside); a lattice edge is crossed iff exactly one end is inside;
+ *   - one vertex per crossed edge, shared by every cell using it, owned by the edge's lower end p and its axis a and
+ *     ordered by (linear index of p, a); t = (iso - v0) / (v1 - v0), q = p with q_a = (float)p_a + t, vertex =
+ *     lo + q * step per axis (fp32, multiply then add, no contraction);
+ *   - triangles ordered by cell linear index (i*(n1-1) + j)*(n2-1) + k, then by the case table's order (tools/mc_table.py:
+ *     generated from a face rule that makes the mesh watertight, at most 5 triangles a cell), counter-clockwise seen from
+ *     outside: the triangle normals point out of the inside region;
+ *   - normals (optional): the volume gradient (central differences, one-sided on the lattice border, divided by step)
+ *     interpolated with t between the edge's ends, negated and normalised; a zero gradient gives (0, 0, 0);
+ *   - no float atomics: two calls are bitwise equal.
+ * The volume is processed in slabs of max(1, NGP_MC_SLAB_POINTS / (n1*n2)) cell planes, so the workspace grows with one
+ * slab, not with the volume. `count` writes {n_vertices, n_triangles} to the device int64[2] `counts`; the caller reads
+ * them back, allocates, and calls `emit` with the same volume, lattice, iso and workspace, nothing else touching the
+ * workspace in between. `emit` checks the capacities against the totals `count` left in the workspace and returns
+ * NGP_EINVAL when they are short, having written nothing: that check is a 16-byte read-back and stream synchronisation,
+ * a second host synchronisation besides the caller's read-back of `counts` (cheap: that one has already drained the
+ * stream), and it makes `emit` unusable under stream capture. Both return NGP_EINVAL for a NULL
+ * pointer (other than normals), an n[a] < 2, n1*n2 > 2^26 or a short workspace. vertices, normals: (V, 3) fp32;
+ * triangles: (F, 3) int64. */
+#define NGP_MC_SLAB_POINTS (1 << 20)
+size_t ngp_marching_cubes_workspace(const NgpLattice* lat); /* bytes; 0 for a lattice the functions reject */
+int ngp_marching_cubes_count(const float* volume, const NgpLattice* lat, float iso, int64_t* counts, void* workspace,
+                             size_t workspace_bytes, void* stream);
+int ngp_marching_cubes_emit(const float* volume, const NgpLattice* lat, float iso, float* vertices, float* normals,
+                            int64_t* triangles, int64_t max_vertices, int64_t max_triangles, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,6 +14,7 @@ ABI_VERSION = 3  # NGP_ABI_VERSION in include/ngp_b200.h
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
 NGP_RGB_MLP_PARAMS = 7168
+NGP_MC_SLAB_POINTS = 1 << 20
 
 
 class NgpGridMeta(C.Structure):
@@ -49,6 +50,15 @@ class NgpSamples(C.Structure):
         ("n_dev", C.c_void_p),
         ("live_idx", C.c_void_p),
         ("n_live_dev", C.c_void_p),
+    ]
+
+
+class NgpLattice(C.Structure):
+    """Mirror of NgpLattice in include/ngp_b200.h."""
+    _fields_ = [
+        ("n", C.c_int32 * 3),
+        ("lo", C.c_float * 3),
+        ("step", C.c_float * 3),
     ]
 
 
@@ -161,6 +171,10 @@ SIGNATURES = {
     "ngp_update_density_grid_eval": (_i, [C.POINTER(NgpNet), _P, _P, _P, _i, _i, _f, _i, _f, _P, _sz, _P]),
     "ngp_image_metrics_workspace": (_sz, [_i, _i]),
     "ngp_image_metrics": (_i, [_P, _P, _i, _i, _i, _f, _P, _P, _P, _sz, _P]),
+    "ngp_density_lattice": (_i, [C.POINTER(NgpNet), C.POINTER(NgpLattice), _P, _P]),
+    "ngp_marching_cubes_workspace": (_sz, [C.POINTER(NgpLattice)]),
+    "ngp_marching_cubes_count": (_i, [_P, C.POINTER(NgpLattice), _f, _P, _P, _sz, _P]),
+    "ngp_marching_cubes_emit": (_i, [_P, C.POINTER(NgpLattice), _f, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
 }
 
 _lib = None

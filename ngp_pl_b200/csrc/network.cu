@@ -377,6 +377,76 @@ extern "C" int ngp_net_forward(const NgpNet* net, const NgpSamples* smp, int wan
 }
 
 // -------------------------------------------------------------------------------------------------
+// density on a lattice (mesh extraction, ngp_pl_b200/mesh.py): k_ngp_fwd's density-only path with the rows generated
+// from the tile index instead of read -- x = lo + (float)idx * step, an fp32 multiply then an fp32 add, so the points
+// are bitwise those a caller materialises with the same formula -- and only sigma written (4 B a point).
+// -------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(FWD_THREADS, FWD_MIN_BLOCKS)
+k_density_lattice(const NgpNet net, const NgpLattice lat, float* __restrict__ sigma) {
+    __shared__ __align__(16) MlpWeightsFwd sw;
+    const __half* wd = reinterpret_cast<const __half*>(net.enc_params_h);
+    load_weights_fwd(sw, wd, nullptr, threadIdx.x, FWD_THREADS);
+    __syncthreads();
+    const uint32_t* table = reinterpret_cast<const uint32_t*>(wd + NGP_DENSITY_MLP_PARAMS);
+
+    const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+    const int64_t n1 = lat.n[1], n2 = lat.n[2];
+    const int64_t n = (int64_t)lat.n[0] * n1 * n2;
+    const int64_t n_tiles = (n + 15) / 16;
+    const int64_t n_warps = (int64_t)gridDim.x * (FWD_THREADS / 32);
+    for (int64_t tile = (int64_t)blockIdx.x * (FWD_THREADS / 32) + (threadIdx.x >> 5); tile < n_tiles; tile += n_warps) {
+        bool valid[1][2];
+        float u[1][2][3];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int64_t row = tile * 16 + g + 8 * h;
+            valid[0][h] = row < n;
+            SampleIn s;
+            s.x = s.y = s.z = 0.f;
+            s.dx = 0.f; s.dy = 0.f; s.dz = 1.f;
+            if (valid[0][h]) {
+                const int64_t k = row % n2, ij = row / n2;
+                const int64_t j = ij % n1, i = ij / n1;
+                s.x = __fadd_rn(lat.lo[0], __fmul_rn((float)i, lat.step[0]));
+                s.y = __fadd_rn(lat.lo[1], __fmul_rn((float)j, lat.step[1]));
+                s.z = __fadd_rn(lat.lo[2], __fmul_rn((float)k, lat.step[2]));
+            }
+            to_unit(net, s, u[0][h][0], u[0][h][1], u[0][h][2]);
+        }
+        uint32_t featA[1][2][4];
+        encode_rows<1>(net, table, u, valid, featA, q);
+        uint32_t hidA[1][4][4];
+        {
+            float hidC[1][8][4];
+            mlp_layer<1, 32, 64, LD32>(featA, sw.w1d, hidC, g, q);
+            relu_to_frag<1, 64>(hidC, hidA);
+        }
+        uint32_t hA[1][1][4];
+        {
+            float hC[1][2][4];
+            mlp_layer<1, 64, 16, LD64>(hidA, sw.w2d, hC, g, q);
+            to_frag<1, 16>(hC, hA);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+            if (valid[0][h] && q == 0) sigma[tile * 16 + g + 8 * h] = expf(lo_half(hA[0][0][h]));
+    }
+}
+
+extern "C" int ngp_density_lattice(const NgpNet* net, const NgpLattice* lat, float* sigma, void* stream) {
+    if (!net || !lat || !sigma || !net->enc_params_h) return NGP_EINVAL;
+    if (net->meta.n_levels < 1 || net->meta.n_levels > NGP_MAX_LEVELS) return NGP_EINVAL;
+    for (int a = 0; a < 3; ++a)
+        if (lat->n[a] < 2) return NGP_EINVAL;
+    const int64_t n = (int64_t)lat->n[0] * lat->n[1] * lat->n[2];
+    const int64_t want = ((n + 15) / 16 + FWD_THREADS / 32 - 1) / (FWD_THREADS / 32);
+    const int64_t cap = (int64_t)ngp_sm_count() * FWD_MIN_BLOCKS;
+    k_density_lattice<<<(int)(want < cap ? want : cap), FWD_THREADS, 0, (cudaStream_t)stream>>>(*net, *lat, sigma);
+    NGP_CHECK_LAUNCH();
+    return 0;
+}
+
+// -------------------------------------------------------------------------------------------------
 // backward: the dgrad chain stays on mma.sync fragments in twelve ROW warps, but the five WEIGHT-GRADIENT GEMMs
 // (dW = dOut^T * In over the 192 staged rows of a block: K = 192, M = 64, N <= 64) are issued by a dedicated MMA WARPGROUP
 // (warps 12-15) as wgmma.mma_async with both operands read from shared memory through matrix descriptors and the fp32
