@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 4
+#define NGP_ABI_VERSION 5
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -351,6 +351,22 @@ int ngp_gen_rays(const int64_t* img_idx, const int64_t* pix_idx, const float* po
 int ngp_sample_rays(const float* poses, const float* directions, const uint8_t* images, int n_img, int64_t n_pix, int n,
                     uint32_t seed, uint32_t stream_id, int32_t* rng_draw, float* rays_o, float* rays_d, float* rgb_gt,
                     float* noise, void* stream);
+
+/* ngp_sample_rays for any bank: image_dtype 0 = uint8 (rgb_gt = v/255, bitwise ngp_sample_rays) or 1 = float32 (rgb_gt = the
+ * stored value); strategy 0 = 'all_images' (bitwise ngp_sample_rays) or 1 = 'same_image' (reference datasets/base.py:27-28:
+ * ONE image per batch, drawn as umulhi(Philox(counter (0, draw, 1, 0)).x, n_img) -- a counter no per-ray draw uses -- while
+ * pixels and jitter are those 'all_images' draws). Other values return NGP_EINVAL. */
+int ngp_sample_rays_ex(const float* poses, const float* directions, const void* images /* (n_img,n_pix,3) */, int image_dtype,
+                       int strategy, int n_img, int64_t n_pix, int n, uint32_t seed, uint32_t stream_id, int32_t* rng_draw,
+                       float* rays_o, float* rays_d, float* rgb_gt, float* noise, void* stream);
+
+/* Image staging (reference datasets/color_utils.py:19-31, read_image(path, (dst_w, dst_h), blend_a)): a decoded uint8
+ * (src_h, src_w, channels) image, channels 3 or 4, becomes fp32 (dst_h*dst_w, 3): v/255 correctly rounded; with 4 channels
+ * c*a + (1-a) (blend_a != 0) or c*a; then cv2.resize's INTER_LINEAR on fp32 when the size changes (a copy otherwise).
+ * Bitwise equal to the reference's arithmetic (oracle/stage_ref.py states the evaluation order). A resize needs
+ * src_h, src_w >= 2. */
+int ngp_stage_image(const uint8_t* src, int src_h, int src_w, int channels, int blend_a, int dst_h, int dst_w, float* dst,
+                    void* stream);
 
 /* Occupancy-grid refresh on the device (reference networks.py:240-269 + :169-195), no host sync:
  * picks cells (all cells when warmup, else M uniform + M occupied per cascade), evaluates sigma at a

@@ -1087,8 +1087,15 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
     return ctr;
 }
 
+__device__ __forceinline__ float image_unit(uint8_t v) { return v * (1.0f / 255.0f); }
+__device__ __forceinline__ float image_unit(float v) { return v; }
+
+// T: the bank's pixel type (uint8 -> v/255, fp32 -> as stored). SAME_IMAGE (reference datasets/base.py:27-28): one image
+// per batch, drawn from the counter (0, draw, 1, 0) -- no per-ray draw has a non-zero third word -- so the pixels and the
+// jitter are those of 'all_images' and only the image index differs.
+template <typename T, bool SAME_IMAGE>
 __global__ void k_sample_rays(const float* __restrict__ poses, const float* __restrict__ directions,
-                              const uint8_t* __restrict__ images, uint32_t n_img, uint32_t n_pix, int n, uint32_t seed,
+                              const T* __restrict__ images, uint32_t n_img, uint32_t n_pix, int n, uint32_t seed,
                               uint32_t stream_id, int* __restrict__ rng_draw, float* __restrict__ rays_o,
                               float* __restrict__ rays_d, float* __restrict__ rgb_gt, float* __restrict__ noise) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1096,7 +1103,12 @@ __global__ void k_sample_rays(const float* __restrict__ poses, const float* __re
     if (i < n) {
         const uint4 r = philox4x32_10(make_uint4((uint32_t)i, draw, 0u, 0u), make_uint2(seed, stream_id));
         // uniform integers by multiply-high (bias < n/2^32), like torch's random_(0, n) up to the generator
-        const uint32_t im = __umulhi(r.x, n_img), px = __umulhi(r.y, n_pix);
+        uint32_t im;
+        if (SAME_IMAGE)
+            im = __umulhi(philox4x32_10(make_uint4(0u, draw, 1u, 0u), make_uint2(seed, stream_id)).x, n_img);
+        else
+            im = __umulhi(r.x, n_img);
+        const uint32_t px = __umulhi(r.y, n_pix);
         noise[i] = (float)(r.z >> 8) * (1.0f / 16777216.0f);
         const float* P = poses + 12 * (size_t)im;
         const float dx = directions[3 * (size_t)px], dy = directions[3 * (size_t)px + 1], dz = directions[3 * (size_t)px + 2];
@@ -1105,10 +1117,10 @@ __global__ void k_sample_rays(const float* __restrict__ poses, const float* __re
             rays_d[3 * i + k] = fmaf(dz, P[4 * k + 2], fmaf(dy, P[4 * k + 1], dx * P[4 * k]));
             rays_o[3 * i + k] = P[4 * k + 3];
         }
-        const uint8_t* c = images + 3 * ((size_t)im * n_pix + px);
-        rgb_gt[3 * i] = c[0] * (1.0f / 255.0f);
-        rgb_gt[3 * i + 1] = c[1] * (1.0f / 255.0f);
-        rgb_gt[3 * i + 2] = c[2] * (1.0f / 255.0f);
+        const T* c = images + 3 * ((size_t)im * n_pix + px);
+        rgb_gt[3 * i] = image_unit(c[0]);
+        rgb_gt[3 * i + 1] = image_unit(c[1]);
+        rgb_gt[3 * i + 2] = image_unit(c[2]);
     }
     // the last block to finish advances the draw counter (every block has read it by then)
     __syncthreads();
@@ -1129,11 +1141,39 @@ extern "C" int ngp_sample_rays(const float* poses, const float* directions, cons
         return NGP_EINVAL;
     if (n == 0) return 0;
     NGP_TRACE(11, (cudaStream_t)stream);
-    k_sample_rays<<<ngp_div_up(n, 256), 256, 0, (cudaStream_t)stream>>>(poses, directions, images, (uint32_t)n_img,
-                                                                         (uint32_t)n_pix, n, seed, stream_id, rng_draw, rays_o,
-                                                                         rays_d, rgb_gt, noise);
+    k_sample_rays<uint8_t, false><<<ngp_div_up(n, 256), 256, 0, (cudaStream_t)stream>>>(
+        poses, directions, images, (uint32_t)n_img, (uint32_t)n_pix, n, seed, stream_id, rng_draw, rays_o, rays_d, rgb_gt, noise);
     NGP_CHECK_LAUNCH();
     NGP_TRACE(1, (cudaStream_t)stream);
+    return 0;
+}
+
+extern "C" int ngp_sample_rays_ex(const float* poses, const float* directions, const void* images, int image_dtype,
+                                  int strategy, int n_img, int64_t n_pix, int n, uint32_t seed, uint32_t stream_id,
+                                  int32_t* rng_draw, float* rays_o, float* rays_d, float* rgb_gt, float* noise, void* stream) {
+    if (n < 0 || n_img < 1 || n_pix < 1 || n_pix > 0xffffffffll || !poses || !directions || !images || !rng_draw || !rays_o ||
+        !rays_d || !rgb_gt || !noise || (image_dtype != 0 && image_dtype != 1) || (strategy != 0 && strategy != 1))
+        return NGP_EINVAL;
+    if (n == 0) return 0;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const dim3 grid(ngp_div_up(n, 256)), block(256);
+    const uint8_t* u8 = (const uint8_t*)images;
+    const float* f32 = (const float*)images;
+    NGP_TRACE(11, st);
+    if (image_dtype == 0 && strategy == 0)
+        k_sample_rays<uint8_t, false><<<grid, block, 0, st>>>(poses, directions, u8, (uint32_t)n_img, (uint32_t)n_pix, n, seed,
+                                                              stream_id, rng_draw, rays_o, rays_d, rgb_gt, noise);
+    else if (image_dtype == 0)
+        k_sample_rays<uint8_t, true><<<grid, block, 0, st>>>(poses, directions, u8, (uint32_t)n_img, (uint32_t)n_pix, n, seed,
+                                                             stream_id, rng_draw, rays_o, rays_d, rgb_gt, noise);
+    else if (strategy == 0)
+        k_sample_rays<float, false><<<grid, block, 0, st>>>(poses, directions, f32, (uint32_t)n_img, (uint32_t)n_pix, n, seed,
+                                                            stream_id, rng_draw, rays_o, rays_d, rgb_gt, noise);
+    else
+        k_sample_rays<float, true><<<grid, block, 0, st>>>(poses, directions, f32, (uint32_t)n_img, (uint32_t)n_pix, n, seed,
+                                                           stream_id, rng_draw, rays_o, rays_d, rgb_gt, noise);
+    NGP_CHECK_LAUNCH();
+    NGP_TRACE(1, st);
     return 0;
 }
 

@@ -104,7 +104,10 @@ class Trainer:
                  T_threshold=1e-4, betas=(0.9, 0.999), eps=1e-15, max_total_samples=None, update_interval=16,
                  warmup_steps=256, process_group=None, world_size=1, rank=0, seed=0, materialize_ws=False, ddp="nccl",
                  lambda_distortion=0.0, skip_dead_samples=True, fused_loss=True, random_bg=False, erode=False,
-                 lr_schedule=None, pick_ahead=True):
+                 lr_schedule=None, pick_ahead=True, ray_sampling_strategy="all_images"):
+        if ray_sampling_strategy not in ("all_images", "same_image"):
+            raise ValueError("Trainer: ray_sampling_strategy must be 'all_images' or 'same_image', got %r" % (ray_sampling_strategy,))
+        self.ray_sampling_strategy = ray_sampling_strategy  # reference opt.py:34-39
         self.model = model
         self.pick_ahead = pick_ahead
         self._picked = None
@@ -411,17 +414,37 @@ class Trainer:
 
     # ---- pieces of one step (all asynchronous) -------------------------------------------------------------
     def attach_bank(self, bank):
-        """bank: synth.RayBank (directions, poses, uint8 images on the device)"""
+        """bank: any object with device tensors `poses` (n,3,4) float32, `directions` (hw,3) float32 and `rgb` (n,hw,3)
+        uint8 (read as v/255) or float32, all contiguous on the trainer's device -- synth.RayBank, datasets.load_scene().
+        Anything else raises."""
+        poses, dirs, rgb = (getattr(bank, k, None) for k in ("poses", "directions", "rgb"))
+        for name, t in (("poses", poses), ("directions", dirs), ("rgb", rgb)):
+            if not isinstance(t, torch.Tensor):
+                raise RuntimeError("Trainer.attach_bank: bank.%s must be a tensor, got %s" % (name, type(t).__name__))
+            if t.device != self.dev:
+                raise RuntimeError("Trainer.attach_bank: bank.%s is on %s, the trainer on %s" % (name, t.device, self.dev))
+            if not t.is_contiguous():
+                raise RuntimeError("Trainer.attach_bank: bank.%s must be contiguous" % name)
+        n, hw = poses.shape[0] if poses.dim() == 3 else -1, dirs.shape[0]
+        if poses.dtype != torch.float32 or poses.dim() != 3 or tuple(poses.shape[1:]) != (3, 4) or n < 1:
+            raise RuntimeError("Trainer.attach_bank: bank.poses must be float32 (n,3,4), got %s %s" % (poses.dtype, tuple(poses.shape)))
+        if dirs.dtype != torch.float32 or dirs.dim() != 2 or dirs.shape[1] != 3 or hw < 1:
+            raise RuntimeError("Trainer.attach_bank: bank.directions must be float32 (hw,3), got %s %s" % (dirs.dtype, tuple(dirs.shape)))
+        if rgb.dtype not in (torch.uint8, torch.float32) or tuple(rgb.shape) != (n, hw, 3):
+            raise RuntimeError("Trainer.attach_bank: bank.rgb must be uint8 or float32 (%d,%d,3), got %s %s"
+                               % (n, hw, rgb.dtype, tuple(rgb.shape)))
         self.bank = bank
 
     def sample_batch(self):
-        """random (image, pixel) pairs with replacement (reference datasets/base.py:22-30) + ray assembly + the march's
-        start jitter, one kernel with a device-side counter-based generator (one stream per buffer set)"""
+        """random (image, pixel) pairs with replacement (reference datasets/base.py:22-30; with 'same_image' one image per
+        batch) + ray assembly + the march's start jitter, one kernel with a device-side counter-based generator (one
+        stream per buffer set)"""
         bk = self.bank
-        rc = _lib.lib().ngp_sample_rays(bk.poses.data_ptr(), bk.directions.data_ptr(), bk.rgb.data_ptr(), bk.poses.shape[0],
-                                        bk.directions.shape[0], self.n_rays, (self.seed * 2654435761 + 97 * self.rank) & 0xffffffff,
-                                        self._cur, self.counters[6:].data_ptr(), self.rays_o.data_ptr(), self.rays_d.data_ptr(),
-                                        self.rgb_gt.data_ptr(), self.noise.data_ptr(), self._st())
+        rc = _lib.lib().ngp_sample_rays_ex(
+            bk.poses.data_ptr(), bk.directions.data_ptr(), bk.rgb.data_ptr(), int(bk.rgb.dtype == torch.float32),
+            int(self.ray_sampling_strategy == "same_image"), bk.poses.shape[0], bk.directions.shape[0], self.n_rays,
+            (self.seed * 2654435761 + 97 * self.rank) & 0xffffffff, self._cur, self.counters[6:].data_ptr(),
+            self.rays_o.data_ptr(), self.rays_d.data_ptr(), self.rgb_gt.data_ptr(), self.noise.data_ptr(), self._st())
         _lib.check(rc, "sample_rays")
 
     def set_batch(self, rays_o, rays_d, rgb_gt):
