@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 5
+#define NGP_ABI_VERSION 6
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -519,6 +519,62 @@ int ngp_marching_cubes_count(const float* volume, const NgpLattice* lat, float i
 int ngp_marching_cubes_emit(const float* volume, const NgpLattice* lat, float iso, float* vertices, float* normals,
                             int64_t* triangles, int64_t max_vertices, int64_t max_triangles, void* workspace,
                             size_t workspace_bytes, void* stream);
+
+/* ----------------------------------------------------------------------------------------------
+ * Test-view images of the validation pass (reference train.py:215-221): `{idx:03d}.png` holds (rgb_pred*255).astype(np.uint8)
+ * and `{idx:03d}_d.png` depth2img(depth) (train.py:45-50; show_gui.py uses it for its depth view), and an 8-bit RGB PNG
+ * encoder for both, so that only the compressed file crosses to the host.
+ * -------------------------------------------------------------------------------------------- */
+#define NGP_VIEW_IMAGES_WORKSPACE 4096 /* bytes, 16-B aligned; no initialisation needed */
+/* rgb (H*W, 3) fp32 and depth (H*W) fp32, as render(test_time=True) returns them -> rgb_img and depth_img, uint8
+ * (H, W, 3), bitwise the reference's arrays:
+ *   rgb_img   = (uint8) trunc(__fmul_rn(v, 255.f)): numpy's cast for every v in [0, 256/255), the range the renderer
+ *               produces; NaN -> 0 as x86 numpy gives. Other values (negative, >= 256/255, inf) are outside the contract:
+ *               they saturate to 0 / 255, which numpy does not promise;
+ *   depth_img = depth2img(depth): mn, mx = the exact min and max over the view (order-free: block partials), NaN
+ *               propagating as numpy's min / max do; idx = trunc(__fmul_rn(__fdiv_rn(__fsub_rn(d, mn), __fsub_rn(mx, mn)),
+ *               255.f)), all float32 as numpy >= 1 computes it; a NaN idx (a constant map's 0/0, or NaN anywhere in the
+ *               view) is 0, as numpy on x86 gives; then the 256-entry table of cv2.applyColorMap(COLORMAP_TURBO)
+ *               (csrc/turbo_table.cuh, generated by tools/turbo_table.py). The channels are cv2's B, G, R in that order:
+ *               the reference hands cv2's BGR array to imageio.imsave as RGB, so its _d.png files hold blue in the red
+ *               position, and so does depth_img. Depths with an infinity are outside the contract.
+ * Either output may be NULL (its input is then not read), not both; workspace is needed with depth_img only.
+ * NGP_EINVAL for H or W < 1, a NULL or non-device pointer that is used, or a short / misaligned workspace.
+ * Two kernels with depth_img (min/max partials, then the images), one without; no synchronisation. */
+int ngp_view_images(const float* rgb, const float* depth, int H, int W, uint8_t* rgb_img, uint8_t* depth_img,
+                    void* workspace, size_t workspace_bytes, void* stream);
+
+/* One complete 8-bit RGB PNG of img (H, W, 3) uint8 (device): signature, IHDR (8-bit, colour type 2, no interlace), one
+ * IDAT, IEND. The file goes to out and its length, an int64, to *out_len -- both written by the device; out and out_len
+ * may be device memory or mapped pinned host memory (cudaHostAlloc; with unified addressing its host pointer is its
+ * device pointer), so only the file's bytes cross PCIe. Nothing in the call synchronises the stream.
+ *
+ * The byte stream is fixed by this algorithm (oracle/png_ref.py restates it byte for byte):
+ *   - Filters, one per row, libpng's heuristic: the type f in None, Sub, Up, Average, Paeth (0..4; bpp 3, the row above
+ *     row 0 is zeros) minimising sum |filtered byte read as int8| over the row's 3W bytes; a tie goes to the lowest f.
+ *     Row r of the filtered stream is the segment [f, filtered bytes], L = 3W + 1 bytes, at stream position r*L.
+ *   - Deflate, one segment per row. A greedy LZ77 parse from the segment's first byte over the candidate distances
+ *     1, 3, L and 2L, a candidate dropped when it exceeds 32768 or reaches before the stream start. At position p the
+ *     match length for d is the number of bytes s[p+i] == s[p-d+i], at most 258 and never past the segment's end; the
+ *     longest wins, a tie to the smaller distance; a length >= 3 is emitted as (length, distance) and the parse skips
+ *     it, otherwise the byte is a literal. The segment is coded as one fixed-Huffman block (BFINAL 0, BTYPE 01, then the
+ *     tokens and end-of-block), or as stored blocks of at most 65535 bytes each (BFINAL 0, BTYPE 00) when those are no
+ *     longer. Either way an empty stored block follows (3 header bits, padding to the byte, LEN 0000, NLEN ffff), so the
+ *     next segment starts on a byte boundary; the last segment's empty block carries BFINAL = 1.
+ *   - Assembly: zlib header 78 01, the segments in row order (offsets from a scan of their byte lengths), the Adler-32
+ *     combined from per-segment (sum d_i, sum (L - i) d_i) pairs in row order. The IDAT CRC-32 is combined from
+ *     per-segment CRCs with crc32_combine (a multiplication by x^(8 len) mod P from a table of x^(2^k)).
+ *   - All arithmetic is integer and fixed-order: two calls give the same bytes.
+ * Sizes: ngp_png_capacity(H, W) = 63 + H * S with S = L + 5 * ceil(L / 65535) + 5 (every segment stored: the largest
+ * file the encoder can write); ngp_png_workspace(H, W) = 256-B-aligned regions for the filtered stream (H*L), the match
+ * table (2 H L), the segments (H * round_up(S, 16)), per-row records (16 H) and offsets (8 H); both are 0 for H or W < 1
+ * or an IDAT that could exceed 2^31 - 1 bytes (6 + H * S). NGP_EINVAL for such a size, a NULL or non-device pointer, a
+ * workspace short or not 256-B aligned, out_len not 8-B aligned, or out_capacity < ngp_png_capacity(H, W).
+ * Four kernels (filter, deflate, assembly, compaction). */
+size_t ngp_png_workspace(int H, int W);
+size_t ngp_png_capacity(int H, int W);
+int ngp_png_encode(const uint8_t* img, int H, int W, uint8_t* out, size_t out_capacity, int64_t* out_len,
+                   void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

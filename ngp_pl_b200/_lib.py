@@ -9,12 +9,13 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 5  #NGP_ABI_VERSION in include/ngp_b200.h
+ABI_VERSION = 6  #NGP_ABI_VERSION in include/ngp_b200.h
 
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
 NGP_RGB_MLP_PARAMS = 7168
 NGP_MC_SLAB_POINTS = 1 << 20
+NGP_VIEW_IMAGES_WORKSPACE = 4096
 
 
 class NgpGridMeta(C.Structure):
@@ -180,6 +181,10 @@ SIGNATURES = {
     "ngp_marching_cubes_workspace": (_sz, [C.POINTER(NgpLattice)]),
     "ngp_marching_cubes_count": (_i, [_P, C.POINTER(NgpLattice), _f, _P, _P, _sz, _P]),
     "ngp_marching_cubes_emit": (_i, [_P, C.POINTER(NgpLattice), _f, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
+    "ngp_view_images": (_i, [_P, _P, _i, _i, _P, _P, _P, _sz, _P]),
+    "ngp_png_workspace": (_sz, [_i, _i]),
+    "ngp_png_capacity": (_sz, [_i, _i]),
+    "ngp_png_encode": (_i, [_P, _i, _i, _P, _sz, _P, _P, _sz, _P]),
 }
 
 _lib = None

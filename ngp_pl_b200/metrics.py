@@ -6,7 +6,8 @@
                                                                     of the reference's --eval_lpips (train.py:65-68, 209-213)
     evaluate(render_fn, poses, directions, images, img_wh, ...)     the validation pass: per-view PSNR and SSIM (and LPIPS
                                                                     given an LpipsNet), gathered over the ranks as
-                                                                    train.py:225-237 does
+                                                                    train.py:225-237 does; with save_dir, the test-view
+                                                                    PNGs of train.py:215-221 (images.py)
 
 The arithmetic is one kernel per view, `ngp_image_metrics` (csrc/metrics.cu), and one `ngp_lpips` chain per view
 (csrc/lpips.cu). Tensors must live on a CUDA device, otherwise RuntimeError; there is no CPU path.
@@ -224,8 +225,8 @@ def gather_metrics(local, n_views, n_pixels, world_size=1, rank=0, process_group
 
 @torch.no_grad()
 def evaluate(render_fn, poses, directions, images, img_wh, world_size=1, rank=0, process_group=None, exp_step_factor=0.0,
-             lpips_net=None):
-    """The reference's validation pass (train.py:193-237) without writing images: renders this rank's share of the views
+             lpips_net=None, save_dir=None):
+    """The reference's validation pass (train.py:193-237): renders this rank's share of the views
     (shard_range, the split bench.py's render_fps uses), runs ngp_image_metrics on each output on the same stream, reads
     the per-view results back once at the end and gathers them over the ranks.
 
@@ -234,7 +235,14 @@ def evaluate(render_fn, poses, directions, images, img_wh, world_size=1, rank=0,
     directions (H*W, 3) (synth.ray_directions); images (n_views, H*W, 3) uint8 (read as v / 255) or float32, or a
     sequence of such views; img_wh = (W, H). Returns {'psnr', 'ssim'} (means over all views), {'psnr_per_view',
     'ssim_per_view'} in view order and 'total_samples' over all views. With lpips_net (an LpipsNet) each view's LPIPS
-    is launched on the same stream after its PSNR and SSIM, and the result gains 'lpips' and 'lpips_per_view'."""
+    is launched on the same stream after its PSNR and SSIM, and the result gains 'lpips' and 'lpips_per_view'.
+
+    With save_dir (created if needed), every view of this rank's shard is also written as the reference's validation
+    pass writes it (train.py:215-221): `{i:03d}.png` = (rgb * 255).astype(uint8) and `{i:03d}_d.png` = depth2img(depth),
+    i the global view index. render_fn's result must then hold 'depth'. Each view's images and PNGs are enqueued on the
+    render stream after its metrics, into a small ring of pinned host slots that one writer thread empties while the GPU
+    renders the next view (images.ViewWriter); the stream is not synchronised per view, the call returns once every file
+    is written, and the returned dict is the one without save_dir."""
     from . import synth
     if isinstance(render_fn, torch.nn.Module):
         from .models.rendering import render
@@ -250,14 +258,26 @@ def evaluate(render_fn, poses, directions, images, img_wh, world_size=1, rank=0,
     local = torch.zeros(hi - lo, 3 if lpips_net is None else 4, dtype=torch.float64, device=dev)
     ws = workspace(H, W, dev)
     ws_lpips = None if lpips_net is None else lpips_workspace(H, W, dev)
-    for i in range(lo, hi):
-        o, d = synth.get_rays(directions, poses[i])
-        res = render_fn(o, d)
-        pred, gt = res["rgb"].float().contiguous(), images[i].contiguous()
-        image_metrics(pred, gt, H, W, local[i - lo, 0], local[i - lo, 1], ws)
-        if lpips_net is not None:
-            lpips_metric(lpips_net, pred, gt, H, W, local[i - lo, 3], ws_lpips)
-        local[i - lo, 2] = res["total_samples"]
+    writer = None
+    if save_dir is not None:
+        from .images import ViewWriter
+        writer = ViewWriter(save_dir, H, W, dev)
+    try:
+        for i in range(lo, hi):
+            o, d = synth.get_rays(directions, poses[i])
+            res = render_fn(o, d)
+            pred, gt = res["rgb"].float().contiguous(), images[i].contiguous()
+            image_metrics(pred, gt, H, W, local[i - lo, 0], local[i - lo, 1], ws)
+            if lpips_net is not None:
+                lpips_metric(lpips_net, pred, gt, H, W, local[i - lo, 3], ws_lpips)
+            local[i - lo, 2] = res["total_samples"]
+            if writer is not None:
+                if "depth" not in res:
+                    raise RuntimeError("ngp_pl_b200.metrics.evaluate: save_dir needs 'depth' in the render result")
+                writer.submit(i, pred, res["depth"].float().contiguous())
+    finally:
+        if writer is not None:
+            writer.close()
     if world_size > 1:
         import torch.distributed as dist
         if dist.get_backend(process_group) != "nccl":
