@@ -14,6 +14,7 @@
 // One round = THREE launches: march, network, compositing (whose last block does the next round's bookkeeping).
 #include "common.cuh"
 #include "march.cuh"
+#include "composite.cuh"
 #include "../../include/ngp_b200.h"
 #include <string.h>
 
@@ -227,23 +228,8 @@ __global__ void k_infer_composite(const NgpInferCfg cfg, const float* __restrict
             const int start = ray_start[i];
             float o = opacity[r], d = depth[r];
             float cr = rgb[3 * r], cg = rgb[3 * r + 1], cb = rgb[3 * r + 2];
-            float T = 1.0f - o;
-            bool term = false;
-            for (int s = 0; s < n; ++s) {
-                const int k = start + s;
-                const float a = 1.0f - __expf(-(__ldg(sigmas + k) * __ldg(deltas + k)));
-                const float w = a * T;
-                cr = fmaf(w, __ldg(rgbs + 3 * k), cr);
-                cg = fmaf(w, __ldg(rgbs + 3 * k + 1), cg);
-                cb = fmaf(w, __ldg(rgbs + 3 * k + 2), cb);
-                d = fmaf(w, __ldg(ts + k), d);
-                o += w;
-                T *= 1.0f - a;
-                if (T <= cfg.T_threshold) {
-                    term = true;
-                    break;
-                }
-            }
+            const bool term = composite_ray_serial(RaySamples{sigmas, deltas, ts, rgbs}, start, n, cfg.T_threshold, cr, cg,
+                                                   cb, d, o);
             opacity[r] = o;
             depth[r] = d;
             rgb[3 * r] = cr; rgb[3 * r + 1] = cg; rgb[3 * r + 2] = cb;

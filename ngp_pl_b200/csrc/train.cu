@@ -80,36 +80,33 @@ __global__ void k_train_march(const NgpTrainCfg cfg, const float* __restrict__ r
     }
 }
 
+// the batch's background colour: per batch from bg_dev (random_bg) or the configured one
+__device__ __forceinline__ float3 batch_bg(const NgpTrainCfg& cfg, const float* bg_dev) {
+    return make_float3(bg_dev ? bg_dev[0] : cfg.bg[0], bg_dev ? bg_dev[1] : cfg.bg[1], bg_dev ? bg_dev[2] : cfg.bg[2]);
+}
+
 // 5. ragged compositing of the network outputs, one warp per ray, + background
 __global__ void k_train_composite_fw(const NgpTrainCfg cfg, const int* __restrict__ n_samples, const int* __restrict__ offsets,
                                      const float* __restrict__ sigmas, const float* __restrict__ rgbs,
                                      const float* __restrict__ deltas, const float* __restrict__ ts,
                                      float* __restrict__ rgb, float* __restrict__ opacity, float* __restrict__ depth,
                                      float* __restrict__ ws, int* __restrict__ counters, const float* __restrict__ bg_dev) {
-    const float bg[3] = {bg_dev ? bg_dev[0] : cfg.bg[0], bg_dev ? bg_dev[1] : cfg.bg[1], bg_dev ? bg_dev[2] : cfg.bg[2]};
+    const float3 bg = batch_bg(cfg, bg_dev);
     const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (w >= cfg.n_rays) return;
     const int64_t start = offsets[w];
     int n = n_samples[w];
     if (start + n > cfg.max_total_samples) n = (int)max((int64_t)0, cfg.max_total_samples - start);
-    const float* sg = sigmas + start;
-    const float* dl = deltas + start;
-    const float* tt = ts + start;
-    const float* cl = rgbs + 3 * start;
-    float* wo = ws ? ws + start : nullptr;
-    const CompositeOut o = composite_ray_warp(
-        n, cfg.T_threshold, lane,
-        [&](int i) { return __ldg(sg + i); }, [&](int i) { return __ldg(dl + i); }, [&](int i) { return __ldg(tt + i); },
-        [&](int i) { return make_float3(__ldg(cl + 3 * i), __ldg(cl + 3 * i + 1), __ldg(cl + 3 * i + 2)); },
-        [&](int i, float v) { if (wo) wo[i] = v; });
+    const RaySamples smp{sigmas + start, deltas + start, ts + start, rgbs + 3 * start};
+    const CompositeOut o = composite_ray_warp<0>(smp, n, cfg.T_threshold, lane, nullptr, ws ? ws + start : nullptr);
     if (lane == 0) {
         const float rest = 1.0f - o.opacity;  // rgb += bg * (1 - opacity), reference rendering.py:160-161
         opacity[w] = o.opacity;
         depth[w] = o.depth;
-        rgb[3 * w] = o.r + bg[0] * rest;
-        rgb[3 * w + 1] = o.g + bg[1] * rest;
-        rgb[3 * w + 2] = o.b + bg[2] * rest;
+        rgb[3 * w] = o.r + bg.x * rest;
+        rgb[3 * w + 1] = o.g + bg.y * rest;
+        rgb[3 * w + 2] = o.b + bg.z * rest;
         if (o.total_samples) atomicAdd(&counters[1], o.total_samples);
     }
 }
@@ -201,7 +198,7 @@ __global__ void k_train_composite_bw(const NgpTrainCfg cfg, const int* __restric
                                      const float* __restrict__ dL_ddepth, const float* __restrict__ dL_dws,
                                      float* __restrict__ dsigmas, float* __restrict__ drgbs, float* __restrict__ amax,
                                      int* __restrict__ live_idx, int* __restrict__ counters, const float* __restrict__ bg_dev) {
-    const float bg[3] = {bg_dev ? bg_dev[0] : cfg.bg[0], bg_dev ? bg_dev[1] : cfg.bg[1], bg_dev ? bg_dev[2] : cfg.bg[2]};
+    const float3 bg = batch_bg(cfg, bg_dev);
     const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (w >= cfg.n_rays) return;
@@ -209,37 +206,20 @@ __global__ void k_train_composite_bw(const NgpTrainCfg cfg, const int* __restric
     int n = n_samples[w];
     if (start + n > cfg.max_total_samples) n = (int)max((int64_t)0, cfg.max_total_samples - start);
     if (n == 0) return;
-    const float* sg = sigmas + start;
-    const float* dl = deltas + start;
-    const float* tt = ts + start;
-    const float* cl = rgbs + 3 * start;
-    const float* wv = ws ? ws + start : nullptr;
-    const float* dw = dL_dws ? dL_dws + start : nullptr;
-    float* ds = dsigmas + start;
-    float* dc = drgbs + 3 * start;
+    const RaySamples smp{sigmas + start, deltas + start, ts + start, rgbs + 3 * start};
     const float3 dC = make_float3(dL_drgb[3 * w], dL_drgb[3 * w + 1], dL_drgb[3 * w + 2]);
     // the forward output is acc + bg*(1-O): undo the background to get the accumulated colour, and
     // route its gradient into the opacity gradient
     const float O = opacity[w];
     const float rest = 1.0f - O;
-    const float3 C = make_float3(rgb[3 * w] - bg[0] * rest, rgb[3 * w + 1] - bg[1] * rest, rgb[3 * w + 2] - bg[2] * rest);
-    const float dO = dL_dopacity[w] - (dC.x * bg[0] + dC.y * bg[1] + dC.z * bg[2]);
+    const float3 C = make_float3(rgb[3 * w] - bg.x * rest, rgb[3 * w + 1] - bg.y * rest, rgb[3 * w + 2] - bg.z * rest);
+    const float dO = dL_dopacity[w] - (dC.x * bg.x + dC.y * bg.y + dC.z * bg.z);
     const float dD = dL_ddepth ? dL_ddepth[w] : 0.f;
-    float m = 0.f;
-    const int n_comp = composite_ray_warp_bwd(
-        n, cfg.T_threshold, lane, dO, dD, dC, O, depth[w], C,
-        [&](int i) { return __ldg(sg + i); }, [&](int i) { return __ldg(dl + i); }, [&](int i) { return __ldg(tt + i); },
-        [&](int i) { return make_float3(__ldg(cl + 3 * i), __ldg(cl + 3 * i + 1), __ldg(cl + 3 * i + 2)); },
-        [&](int i) { return dw ? __ldg(dw + i) : 0.f; }, [&](int i) { return (dw && wv) ? __ldg(wv + i) : 0.f; },
-        [&](int i, float v) {
-            ds[i] = v;
-            m = fmaxf(m, fabsf(v * fminf(__ldg(sg + i), 3.2690173e6f)));
-        },
-        [&](int i, float3 v) {
-            dc[3 * i] = v.x; dc[3 * i + 1] = v.y; dc[3 * i + 2] = v.z;
-            m = fmaxf(m, fmaxf(fabsf(v.x), fmaxf(fabsf(v.y), fabsf(v.z))));
-        });
-    m = warp_max(m);
+    const CompositeBwdOut g = composite_ray_warp_bwd<0, true>(smp, n, cfg.T_threshold, lane, nullptr, dC, dO, dD, C, O,
+                                                              depth[w], dL_dws ? dL_dws + start : nullptr,
+                                                              ws ? ws + start : nullptr, dsigmas + start, drgbs + 3 * start);
+    const int n_comp = g.n_composited;
+    const float m = warp_max(g.m);
     if (lane == 0 && m > 0.f && m < INFINITY) atomicMax(reinterpret_cast<int*>(amax), __float_as_int(m));
     // the composited samples are the ray's leading n_comp: append them to the list the network backward visits
     // (every other sample has dsigmas = drgbs = 0 exactly and would only add zeros)
@@ -283,19 +263,6 @@ __global__ void k_train_grad_scale(float* __restrict__ scalars, int* __restrict_
 // without the two extra launches and with the second sweep over the ray's samples hitting L1/L2.
 #define CL_WARPS 8  // rays per block of k_train_composite_loss
 #define CL_CACHE 4  // trips (of 32 samples) of a ray held in registers between the forward and the backward sweep (64 regs)
-struct CLSample {
-    float sg, de, ti;
-    float3 c;
-};
-__device__ __forceinline__ CLSample cl_load(const float* __restrict__ sg, const float* __restrict__ dl,
-                                            const float* __restrict__ tt, const float* __restrict__ cl, int i) {
-    CLSample x;
-    x.sg = __ldg(sg + i);
-    x.de = __ldg(dl + i);
-    x.ti = __ldg(tt + i);
-    x.c = make_float3(__ldg(cl + 3 * i), __ldg(cl + 3 * i + 1), __ldg(cl + 3 * i + 2));
-    return x;
-}
 __global__ void __launch_bounds__(CL_WARPS * 32) k_train_composite_loss(const NgpTrainCfg cfg, const int* __restrict__ n_samples, const int* __restrict__ offsets,
                                        const float* __restrict__ sigmas, const float* __restrict__ rgbs,
                                        const float* __restrict__ deltas, const float* __restrict__ ts,
@@ -303,7 +270,7 @@ __global__ void __launch_bounds__(CL_WARPS * 32) k_train_composite_loss(const Ng
                                        float* __restrict__ depth, float* __restrict__ dsigmas, float* __restrict__ drgbs,
                                        float* __restrict__ scalars, int* __restrict__ live_idx, int* __restrict__ counters,
                                        const float* __restrict__ bg_dev) {
-    const float bg[3] = {bg_dev ? bg_dev[0] : cfg.bg[0], bg_dev ? bg_dev[1] : cfg.bg[1], bg_dev ? bg_dev[2] : cfg.bg[2]};
+    const float3 bg = batch_bg(cfg, bg_dev);
     const int lane = threadIdx.x & 31;
     // (n_rays is a multiple of the rays per block or the last block's spare warps idle on ray n_rays - 1 with n = 0 and
     // contribute nothing: every warp must reach the block barriers below)
@@ -313,72 +280,21 @@ __global__ void __launch_bounds__(CL_WARPS * 32) k_train_composite_loss(const Ng
     const int64_t start = offsets[w];
     int n = real ? n_samples[w] : 0;
     if (start + n > cfg.max_total_samples) n = (int)max((int64_t)0, cfg.max_total_samples - start);
-    const float* sg = sigmas + start;
-    const float* dl = deltas + start;
-    const float* tt = ts + start;
-    const float* cl = rgbs + 3 * start;
+    const RaySamples smp{sigmas + start, deltas + start, ts + start, rgbs + 3 * start};
     // The ray's first CL_CACHE trips of 32 samples are loaded up front (independent loads, one exposed latency instead of
     // one per trip) and kept in registers for the backward sweep; longer rays continue trip by trip from memory. The
-    // kernel is two waves of warps and lasts as long as its longest rays: with the generic helpers (a dependent load ->
-    // scan chain per trip, twice) those chains were what it waited on. Arithmetic and its order are those of
-    // composite_ray_warp / composite_ray_warp_bwd (composite.cuh), minus the depth and ws scans whose gradients are zero.
+    // kernel is two waves of warps and lasts as long as its longest rays: without the cache (a dependent load -> scan
+    // chain per trip, twice) those chains were what it waited on. The sweeps are those of k_train_composite_fw /
+    // k_train_composite_bw (composite.cuh), minus the depth and ws scans whose gradients are zero.
     CLSample sm[CL_CACHE];
 #pragma unroll
-    for (int k = 0; k < CL_CACHE; ++k) {
-        const int i = k * 32 + lane;
-        sm[k].sg = 0.f; sm[k].de = 0.f; sm[k].ti = 0.f; sm[k].c = make_float3(0.f, 0.f, 0.f);
-        if (i < n) sm[k] = cl_load(sg, dl, tt, cl, i);
-    }
-    CompositeOut o;
-    {
-        float acc_r = 0.f, acc_g = 0.f, acc_b = 0.f, acc_d = 0.f, acc_o = 0.f, T_carry = 1.0f;
-        int n_comp = 0;
-        bool done = false;
-        auto trip = [&](int base, const CLSample& x) {
-            const int i = base + lane;
-            const bool valid = i < n;
-            const float a = valid ? 1.0f - __expf(-(x.sg * x.de)) : 0.f;
-            const float T_inc = warp_scan_mul(1.0f - a, lane) * T_carry;
-            float T_exc = __shfl_up_sync(0xffffffffu, T_inc, 1);
-            if (lane == 0) T_exc = T_carry;
-            const bool comp = valid && (i == 0 || T_exc > cfg.T_threshold);
-            const float w = comp ? a * T_exc : 0.f;
-            if (comp) {
-                acc_r = fmaf(w, x.c.x, acc_r);
-                acc_g = fmaf(w, x.c.y, acc_g);
-                acc_b = fmaf(w, x.c.z, acc_b);
-                acc_d = fmaf(w, x.ti, acc_d);
-                acc_o += w;
-            }
-            n_comp += __popc(__ballot_sync(0xffffffffu, comp));
-            done = __ballot_sync(0xffffffffu, valid && !(T_inc > cfg.T_threshold)) != 0u;
-            T_carry = __shfl_sync(0xffffffffu, T_inc, 31);
-        };
-#pragma unroll
-        for (int k = 0; k < CL_CACHE; ++k)
-            if (k * 32 < n && !done) trip(k * 32, sm[k]);
-        for (int base = CL_CACHE * 32; base < n && !done; base += 32) {
-            CLSample x;
-            x.sg = 0.f; x.de = 0.f; x.ti = 0.f; x.c = make_float3(0.f, 0.f, 0.f);
-            if (base + lane < n) x = cl_load(sg, dl, tt, cl, base + lane);
-            trip(base, x);
-        }
-        o.r = warp_sum(acc_r);
-        o.g = warp_sum(acc_g);
-        o.b = warp_sum(acc_b);
-        o.depth = warp_sum(acc_d);
-        o.opacity = warp_sum(acc_o);
-        o.n_composited = n_comp;
-        o.total_samples = done ? n_comp - 1 : n_comp;
-    }
+    for (int k = 0; k < CL_CACHE; ++k) cl_load(sm[k], smp, k * 32 + lane, n);
+    const CompositeOut o = composite_ray_warp<CL_CACHE>(smp, n, cfg.T_threshold, lane, sm, nullptr);
     const float rest = 1.0f - o.opacity;  // rgb += bg * (1 - opacity), reference rendering.py:160-161
-    const float3 out = make_float3(o.r + bg[0] * rest, o.g + bg[1] * rest, o.b + bg[2] * rest);
-    // NeRFLoss (reference losses.py:47-60, lambda_distortion = 0) and its per-ray gradients
+    const float3 out = make_float3(o.r + bg.x * rest, o.g + bg.y * rest, o.b + bg.z * rest);
     const float inv_n = 1.0f / (float)cfg.n_rays;
-    const float ex = out.x - rgb_gt[3 * w], ey = out.y - rgb_gt[3 * w + 1], ez = out.z - rgb_gt[3 * w + 2];
-    const float3 dC = make_float3(2.0f * ex * inv_n * (1.0f / 3.0f), 2.0f * ey * inv_n * (1.0f / 3.0f), 2.0f * ez * inv_n * (1.0f / 3.0f));
-    const float op = o.opacity + 1e-10f;
-    const float lg = logf(op);
+    const NerfLossRay l = nerf_loss_ray(out, make_float3(rgb_gt[3 * w], rgb_gt[3 * w + 1], rgb_gt[3 * w + 2]), o.opacity,
+                                        cfg.lambda_opacity, inv_n);
     if (lane == 0 && real) {
         opacity[w] = o.opacity;
         depth[w] = o.depth;
@@ -388,61 +304,12 @@ __global__ void __launch_bounds__(CL_WARPS * 32) k_train_composite_loss(const Ng
     float m = 0.f;
     int n_comp = 0;
     if (n > 0) {
-        const float dO = cfg.lambda_opacity * (-lg - 1.0f) * inv_n - (dC.x * bg[0] + dC.y * bg[1] + dC.z * bg[2]);
-        float* ds = dsigmas + start;
-        float* dc = drgbs + 3 * start;
-        const float3 C = make_float3(o.r, o.g, o.b);
-        const float dO_term = dO * (1.0f - o.opacity);
-        float T_carry = 1.0f, pr = 0.f, pg = 0.f, pb = 0.f;
-        bool done = false;
-        auto trip = [&](int base, const CLSample& x) {
-            const int i = base + lane;
-            const bool valid = i < n;
-            const float a = valid ? 1.0f - __expf(-(x.sg * x.de)) : 0.f;
-            const float T_inc = warp_scan_mul(1.0f - a, lane) * T_carry;
-            float T_exc = __shfl_up_sync(0xffffffffu, T_inc, 1);
-            if (lane == 0) T_exc = T_carry;
-            const bool comp = valid && (i == 0 || T_exc > cfg.T_threshold);
-            const float w = comp ? a * T_exc : 0.f;
-            const float r_inc = warp_scan_add(w * x.c.x, lane) + pr;
-            const float g_inc = warp_scan_add(w * x.c.y, lane) + pg;
-            const float b_inc = warp_scan_add(w * x.c.z, lane) + pb;
-            if (valid) {
-                float3 dcv = make_float3(0.f, 0.f, 0.f);
-                float dsv = 0.f;
-                if (comp) {
-                    dcv = make_float3(dC.x * w, dC.y * w, dC.z * w);
-                    const float g = dC.x * (x.c.x * T_inc - (C.x - r_inc)) + dC.y * (x.c.y * T_inc - (C.y - g_inc)) +
-                                    dC.z * (x.c.z * T_inc - (C.z - b_inc)) + dO_term;
-                    dsv = x.de * g;
-                }
-                dc[3 * i] = dcv.x; dc[3 * i + 1] = dcv.y; dc[3 * i + 2] = dcv.z;
-                ds[i] = dsv;
-                m = fmaxf(m, fmaxf(fabsf(dcv.x), fmaxf(fabsf(dcv.y), fabsf(dcv.z))));
-                m = fmaxf(m, fabsf(dsv * fminf(x.sg, 3.2690173e6f)));
-            }
-            n_comp += __popc(__ballot_sync(0xffffffffu, comp));
-            done = __ballot_sync(0xffffffffu, valid && !(T_inc > cfg.T_threshold)) != 0u;
-            T_carry = __shfl_sync(0xffffffffu, T_inc, 31);
-            pr = __shfl_sync(0xffffffffu, r_inc, 31);
-            pg = __shfl_sync(0xffffffffu, g_inc, 31);
-            pb = __shfl_sync(0xffffffffu, b_inc, 31);
-        };
-        int base = 0;
-#pragma unroll
-        for (int k = 0; k < CL_CACHE; ++k)
-            if (k * 32 < n && !done) { trip(k * 32, sm[k]); base = k * 32 + 32; }
-        for (; base >= CL_CACHE * 32 && base < n && !done; base += 32) {
-            CLSample x;
-            x.sg = 0.f; x.de = 0.f; x.ti = 0.f; x.c = make_float3(0.f, 0.f, 0.f);
-            if (base + lane < n) x = cl_load(sg, dl, tt, cl, base + lane);
-            trip(base, x);
-        }
-        for (int i = base + lane; i < n; i += 32) {  // past the terminating trip: zero gradients
-            dc[3 * i] = 0.f; dc[3 * i + 1] = 0.f; dc[3 * i + 2] = 0.f;
-            ds[i] = 0.f;
-        }
-        m = warp_max(m);
+        const float dO = __fmaf_rn(l.dO_n, inv_n, -(l.dC.x * bg.x + l.dC.y * bg.y + l.dC.z * bg.z));
+        const CompositeBwdOut g = composite_ray_warp_bwd<CL_CACHE, false>(
+            smp, n, cfg.T_threshold, lane, sm, l.dC, dO, 0.f, make_float3(o.r, o.g, o.b), o.opacity, o.depth, nullptr,
+            nullptr, dsigmas + start, drgbs + 3 * start);
+        n_comp = g.n_composited;
+        m = warp_max(g.m);
     }
     // Per-ray sums, the loss-scale maximum and the live-list allocation go through ONE set of atomics per BLOCK (8 rays):
     // five same-address atomics per ray serialise in the L2 atomic unit.
@@ -450,8 +317,8 @@ __global__ void __launch_bounds__(CL_WARPS * 32) k_train_composite_loss(const Ng
     __shared__ int s_tot[CL_WARPS], s_comp[CL_WARPS], s_base;
     const int wib = threadIdx.x >> 5;
     if (lane == 0) {
-        s_se[wib] = ex * ex + ey * ey + ez * ez;
-        s_ent[wib] = -op * lg;
+        s_se[wib] = l.se;
+        s_ent[wib] = l.ent;
         s_m[wib] = (m > 0.f && m < INFINITY) ? m : 0.f;
         s_tot[wib] = o.total_samples;
         s_comp[wib] = n_comp;
@@ -552,16 +419,13 @@ __global__ void k_nerf_loss_grad(const NgpTrainCfg cfg, const float* __restrict_
     float se = 0.f, ent = 0.f;
     if (r < cfg.n_rays) {
         const float inv_n = 1.0f / (float)cfg.n_rays;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const float e = rgb[3 * r + c] - rgb_gt[3 * r + c];
-            se += e * e;
-            dL_drgb[3 * r + c] = 2.0f * e * inv_n * (1.0f / 3.0f);
-        }
-        const float o = opacity[r] + 1e-10f;
-        const float lg = logf(o);
-        ent = -o * lg;
-        dL_dopacity[r] = cfg.lambda_opacity * (-lg - 1.0f) * inv_n;
+        const NerfLossRay l = nerf_loss_ray(make_float3(rgb[3 * r], rgb[3 * r + 1], rgb[3 * r + 2]),
+                                            make_float3(rgb_gt[3 * r], rgb_gt[3 * r + 1], rgb_gt[3 * r + 2]), opacity[r],
+                                            cfg.lambda_opacity, inv_n);
+        dL_drgb[3 * r] = l.dC.x; dL_drgb[3 * r + 1] = l.dC.y; dL_drgb[3 * r + 2] = l.dC.z;
+        dL_dopacity[r] = l.dO_n * inv_n;
+        se = l.se;
+        ent = l.ent;
     }
     se = warp_sum(se);
     ent = warp_sum(ent);

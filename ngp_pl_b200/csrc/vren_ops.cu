@@ -485,16 +485,8 @@ __global__ void k_composite_train_fw(const float* __restrict__ sigmas, const flo
     const int64_t ray = rays_a[3 * w];
     const int64_t start = rays_a[3 * w + 1];
     const int n = (int)rays_a[3 * w + 2];
-    const float* sg = sigmas + start;
-    const float* dl = deltas + start;
-    const float* tt = ts + start;
-    const float* cl = rgbs + 3 * start;
-    float* wo = ws + start;
-    const CompositeOut o = composite_ray_warp(
-        n, T_threshold, lane,
-        [&](int i) { return __ldg(sg + i); }, [&](int i) { return __ldg(dl + i); }, [&](int i) { return __ldg(tt + i); },
-        [&](int i) { return make_float3(__ldg(cl + 3 * i), __ldg(cl + 3 * i + 1), __ldg(cl + 3 * i + 2)); },
-        [&](int i, float v) { wo[i] = v; });
+    const RaySamples smp{sigmas + start, deltas + start, ts + start, rgbs + 3 * start};
+    const CompositeOut o = composite_ray_warp<0>(smp, n, T_threshold, lane, nullptr, ws + start);
     if (lane == 0) {
         opacity[ray] = o.opacity;
         depth[ray] = o.depth;
@@ -532,23 +524,12 @@ __global__ void k_composite_train_bw(const float* __restrict__ dL_dopacity, cons
     const int64_t ray = rays_a[3 * w];
     const int64_t start = rays_a[3 * w + 1];
     const int n = (int)rays_a[3 * w + 2];
-    const float* sg = sigmas + start;
-    const float* dl = deltas + start;
-    const float* tt = ts + start;
-    const float* cl = rgbs + 3 * start;
-    const float* wv = ws + start;
-    const float* dw = dL_dws + start;
-    float* ds = dL_dsigmas + start;
-    float* dc = dL_drgbs + 3 * start;
-    composite_ray_warp_bwd(
-        n, T_threshold, lane, dL_dopacity[ray], dL_ddepth[ray],
-        make_float3(dL_drgb[3 * ray], dL_drgb[3 * ray + 1], dL_drgb[3 * ray + 2]),
-        opacity[ray], depth[ray], make_float3(rgb[3 * ray], rgb[3 * ray + 1], rgb[3 * ray + 2]),
-        [&](int i) { return __ldg(sg + i); }, [&](int i) { return __ldg(dl + i); }, [&](int i) { return __ldg(tt + i); },
-        [&](int i) { return make_float3(__ldg(cl + 3 * i), __ldg(cl + 3 * i + 1), __ldg(cl + 3 * i + 2)); },
-        [&](int i) { return __ldg(dw + i); }, [&](int i) { return __ldg(wv + i); },
-        [&](int i, float v) { ds[i] = v; },
-        [&](int i, float3 v) { dc[3 * i] = v.x; dc[3 * i + 1] = v.y; dc[3 * i + 2] = v.z; });
+    const RaySamples smp{sigmas + start, deltas + start, ts + start, rgbs + 3 * start};
+    composite_ray_warp_bwd<0, true>(smp, n, T_threshold, lane, nullptr,
+                                    make_float3(dL_drgb[3 * ray], dL_drgb[3 * ray + 1], dL_drgb[3 * ray + 2]),
+                                    dL_dopacity[ray], dL_ddepth[ray],
+                                    make_float3(rgb[3 * ray], rgb[3 * ray + 1], rgb[3 * ray + 2]), opacity[ray],
+                                    depth[ray], dL_dws + start, ws + start, dL_dsigmas + start, dL_drgbs + 3 * start);
 }
 
 extern "C" int ngp_composite_train_bw(const float* dL_dopacity, const float* dL_ddepth, const float* dL_drgb,
@@ -586,23 +567,8 @@ __global__ void k_composite_test_fw(const float* __restrict__ sigmas, const floa
     const int64_t r = alive[n];
     float o = opacity[r], d = depth[r];
     float cr = rgb[3 * r], cg = rgb[3 * r + 1], cb = rgb[3 * r + 2];
-    float T = 1.0f - o;
     const int64_t row = (int64_t)n * n_samples_max;
-    for (int s = 0; s < ne; ++s) {
-        const int64_t k = row + s;
-        const float a = 1.0f - __expf(-(sigmas[k] * deltas[k]));
-        const float w = a * T;
-        cr = fmaf(w, rgbs[3 * k], cr);
-        cg = fmaf(w, rgbs[3 * k + 1], cg);
-        cb = fmaf(w, rgbs[3 * k + 2], cb);
-        d = fmaf(w, ts[k], d);
-        o += w;
-        T *= 1.0f - a;
-        if (T <= T_threshold) {
-            alive[n] = -1;
-            break;
-        }
-    }
+    if (composite_ray_serial(RaySamples{sigmas, deltas, ts, rgbs}, row, ne, T_threshold, cr, cg, cb, d, o)) alive[n] = -1;
     opacity[r] = o;
     depth[r] = d;
     rgb[3 * r] = cr; rgb[3 * r + 1] = cg; rgb[3 * r + 2] = cb;
