@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 6
+#define NGP_ABI_VERSION 7
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -575,6 +575,46 @@ size_t ngp_png_workspace(int H, int W);
 size_t ngp_png_capacity(int H, int W);
 int ngp_png_encode(const uint8_t* img, int H, int W, uint8_t* out, size_t out_capacity, int64_t* out_len,
                    void* workspace, size_t workspace_bytes, void* stream);
+
+/* One complete baseline JPEG of img (H, W, 3) uint8 RGB (device), for the Motion-JPEG videos of the test views. As with
+ * ngp_png_encode the file goes to out and its length, an int64, to *out_len, both written by the device; out and out_len
+ * may be device memory or mapped pinned host memory; nothing in the call synchronises the stream.
+ *
+ * One fixed format; quality (1..100) is the only choice. The byte stream (oracle/jpeg_ref.py restates it byte for byte,
+ * and it is the file libjpeg writes for the same quality with 4:4:4 sampling, its default tables and its accurate
+ * integer DCT, e.g. Pillow's save(quality=q, subsampling=0, optimize=False)):
+ *   - Segments: SOI; APP0 JFIF 1.01, density unit 0, 1 x 1, no thumbnail; DQT table 0; DQT table 1 (8-bit entries in
+ *     zig-zag order); SOF0 (baseline sequential DCT, 8-bit, H, W, components 1, 2, 3 = Y, Cb, Cr, each sampled 1 x 1,
+ *     quantisation tables 0, 1, 1); DHT DC 0, AC 0, DC 1, AC 1: the "typical" tables of ITU-T T.81 Annex K.3; SOS (one
+ *     interleaved scan, Huffman tables 0, 1, 1, coefficients 0..63); the entropy-coded data; EOI. No restart intervals.
+ *     The segments before the data are 623 bytes.
+ *   - Quantisation tables: the Annex K.1 luminance and chrominance tables scaled as libjpeg does, s = 5000 / quality
+ *     below 50 and 200 - 2 quality from 50, entry = (base * s + 50) / 100 in integers, clamped to 1..255.
+ *   - Colour: Y = (19595 R + 38470 G + 7471 B + 32768) >> 16, Cb = (-11059 R - 21709 G + 32768 B + 8421375) >> 16,
+ *     Cr = (32768 R - 27439 G - 5329 B + 8421375) >> 16 (8421375 = (128 << 16) + 32767). The image is cut into 8 x 8
+ *     blocks, the last column and row repeated up to a multiple of 8; 128 is subtracted from every sample.
+ *   - Forward DCT: the Loeffler-Ligtenberg-Moschytz factorisation in 32-bit integers with 13-bit constants, rows then
+ *     columns, the row pass scaled up by 4 and every product sum rounded by adding half before the arithmetic shift;
+ *     the block comes out scaled by 8. Quantisation: sign(c) * ((|c| + 4 q) / (8 q)), i.e. rounding half away from zero.
+ *   - Entropy coding: an MCU is the Y, Cb, Cr blocks of one 8 x 8 area, MCUs in raster order. Per block: the difference
+ *     of the DC coefficient to the same component's DC of the previous MCU (0 before the first) as its size category's
+ *     code and that many magnitude bits (a negative value v as the low bits of v - 1); the AC coefficients in zig-zag
+ *     order as run/size codes with magnitude bits, a run over 15 as ZRL codes, and EOB unless coefficient 63 is not
+ *     zero. Bits are packed most significant first, the last byte is filled with 1-bits, and every 0xFF byte of the
+ *     data is followed by a 0x00.
+ *   - All arithmetic is integer and order-free (codes are OR-ed into a zeroed stream): two calls give the same bytes.
+ * Sizes, with B = 3 * ceil(H / 8) * ceil(W / 8) blocks: a block codes to at most 20 + 63 * 26 = 1658 bits, taken as 208
+ * bytes, and stuffing at most doubles them, so ngp_jpeg_capacity(H, W) = 623 + 416 B + 2. ngp_jpeg_workspace(H, W) =
+ * 256-B-aligned regions for the coefficients (128 B), per-MCU bit counts (4 B / 3), the unstuffed stream (208 B + 8
+ * rounded up to 512) and per-512-byte 0xFF counts, plus 256 bytes. Both are 0 for H or W outside 1..65535 (the SOF0
+ * fields) or 1664 B > 2^31 - 1 (bit offsets are 32-bit: about 27 million pixels). NGP_EINVAL for such a size, a quality
+ * outside 1..100, a NULL or non-device pointer, a workspace short or not 256-B aligned, out_len not 8-B aligned, or
+ * out_capacity < ngp_jpeg_capacity(H, W). One memset of the stream and seven kernels (DCT, bit counts, scan, code
+ * emission, 0xFF counts, scan, stuffing and assembly). */
+size_t ngp_jpeg_workspace(int H, int W);
+size_t ngp_jpeg_capacity(int H, int W);
+int ngp_jpeg_encode(const uint8_t* img, int H, int W, int quality, uint8_t* out, size_t out_capacity, int64_t* out_len,
+                    void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -9,7 +9,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 6  #NGP_ABI_VERSION in include/ngp_b200.h
+ABI_VERSION = 7  #NGP_ABI_VERSION in include/ngp_b200.h
 
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
@@ -185,6 +185,9 @@ SIGNATURES = {
     "ngp_png_workspace": (_sz, [_i, _i]),
     "ngp_png_capacity": (_sz, [_i, _i]),
     "ngp_png_encode": (_i, [_P, _i, _i, _P, _sz, _P, _P, _sz, _P]),
+    "ngp_jpeg_workspace": (_sz, [_i, _i]),
+    "ngp_jpeg_capacity": (_sz, [_i, _i]),
+    "ngp_jpeg_encode": (_i, [_P, _i, _i, _i, _P, _sz, _P, _P, _sz, _P]),
 }
 
 _lib = None

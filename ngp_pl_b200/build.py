@@ -15,7 +15,7 @@ INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libngp_b200.so")
 
-SOURCES = ["vren_ops.cu", "network.cu", "train.cu", "infer.cu", "modules.cu", "metrics.cu", "mesh.cu", "lpips.cu", "stage.cu", "images.cu"]
+SOURCES = ["vren_ops.cu", "network.cu", "train.cu", "infer.cu", "modules.cu", "metrics.cu", "mesh.cu", "lpips.cu", "stage.cu", "images.cu", "jpeg.cu"]
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",

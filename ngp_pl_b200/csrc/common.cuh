@@ -60,6 +60,19 @@ static inline int ngp_sm_count() {
     return sms;
 }
 
+// Whether the device can address p: device or managed memory, or (host_mapped_ok) mapped pinned host memory whose host
+// pointer is its device pointer.
+static inline bool ngp_dev_ptr(const void* p, bool host_mapped_ok) {
+    if (!p) return false;
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();  // a failed query is not an error of the next launch
+        return false;
+    }
+    if (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) return true;
+    return host_mapped_ok && a.type == cudaMemoryTypeHost && a.devicePointer == p;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

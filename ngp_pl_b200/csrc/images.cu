@@ -560,17 +560,6 @@ bool png_layout(int H, int W, PngLayout& y) {
     return true;
 }
 
-bool dev_ptr(const void* p, bool host_mapped_ok) {
-    if (!p) return false;
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-        cudaGetLastError();  // a failed query is not an error of the next launch
-        return false;
-    }
-    if (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) return true;
-    return host_mapped_ok && a.type == cudaMemoryTypeHost && a.devicePointer == p;
-}
-
 int grid_for(int64_t n_rows) { return (int)std::min<int64_t>((n_rows + PNG_WARPS - 1) / PNG_WARPS, 32LL * ngp_sm_count()); }
 
 }  // namespace
@@ -578,8 +567,8 @@ int grid_for(int64_t n_rows) { return (int)std::min<int64_t>((n_rows + PNG_WARPS
 extern "C" int ngp_view_images(const float* rgb, const float* depth, int H, int W, uint8_t* rgb_img, uint8_t* depth_img,
                                void* workspace, size_t workspace_bytes, void* stream) {
     if (H < 1 || W < 1 || (!rgb_img && !depth_img)) return NGP_EINVAL;
-    if (rgb_img && (!dev_ptr(rgb, false) || !dev_ptr(rgb_img, false))) return NGP_EINVAL;
-    if (depth_img && (!dev_ptr(depth, false) || !dev_ptr(depth_img, false) || !dev_ptr(workspace, false) ||
+    if (rgb_img && (!ngp_dev_ptr(rgb, false) || !ngp_dev_ptr(rgb_img, false))) return NGP_EINVAL;
+    if (depth_img && (!ngp_dev_ptr(depth, false) || !ngp_dev_ptr(depth_img, false) || !ngp_dev_ptr(workspace, false) ||
                       workspace_bytes < NGP_VIEW_IMAGES_WORKSPACE || ((uintptr_t)workspace & 15)))
         return NGP_EINVAL;
     const cudaStream_t st = (cudaStream_t)stream;
@@ -611,7 +600,7 @@ extern "C" int ngp_png_encode(const uint8_t* img, int H, int W, uint8_t* out, si
                               void* workspace, size_t workspace_bytes, void* stream) {
     PngLayout y;
     if (!png_layout(H, W, y)) return NGP_EINVAL;
-    if (!dev_ptr(img, false) || !dev_ptr(workspace, false) || !dev_ptr(out, true) || !dev_ptr(out_len, true))
+    if (!ngp_dev_ptr(img, false) || !ngp_dev_ptr(workspace, false) || !ngp_dev_ptr(out, true) || !ngp_dev_ptr(out_len, true))
         return NGP_EINVAL;
     if (workspace_bytes < (size_t)y.total || out_capacity < ngp_png_capacity(H, W) || ((uintptr_t)workspace & 255) ||
         ((uintptr_t)out_len & 7))
