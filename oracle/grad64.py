@@ -1,4 +1,4 @@
-"""float64 restatement of the network backward and of the hash-table scatter -- TEST INFRASTRUCTURE ONLY.
+"""float64 restatement of the network forward, the network backward and the hash-table scatter -- TEST INFRASTRUCTURE ONLY.
 
 Nothing under ngp_pl_b200/ imports this. It is plain torch (any device), so the GPU tests run it on CUDA at training
 sizes and the CPU suite checks it against oracle.torch_ngp_forward / torch_grid_encode on small inputs.
@@ -22,6 +22,11 @@ Every value comes with a rigorous bound of how far the kernel's may lie from it 
 A row whose ReLU masks are not determined by those intervals is flagged in `ambiguous`: there the kernel and the
 reference may take different branches and no rounding bound applies. `ambiguous_own` flags the subset where the
 pre-activation's own accumulation error alone (|z| <= 2^-20 sum|terms|) leaves the mask open.
+
+mlp_forward() is that forward on its own, as intervals (with carry=True every bound is followed to the outputs);
+grid_encode(), sigma(), sh_encode(), ray_positions() and to_unit() restate the rest of k_ngp_fwd / k_sh_encode: the
+hash-grid features, sigma = expf(h0), the stand-alone SH encoding and the sample positions, each with its derived bound
+(or bit for bit where the arithmetic allows).
 
 grid_scatter() restates k_grid_scatter_merged: corner weights in float32 exactly as grid_cell / grid_corner_weights
 compute them (bit for bit), indices as grid_corner_indices (dense wrap included), contributions w g / scale summed in
@@ -83,15 +88,19 @@ def _rounded(y, e, relu):
     return a, torch.maximum(hi - a, a - lo), amb
 
 
-def _fwd(x, dx, W, relu):
+def _fwd(x, dx, W, relu, carry=False):
     """one forward layer from inputs the kernel may have rounded differently by up to dx: the fp16 output, by how much the
-    kernel's may differ (one ulp where its own fp32 accumulation error straddles a rounding boundary) and, for a ReLU,
-    the rows whose mask the accumulation error together with dx leaves undetermined"""
+    kernel's may differ (one ulp where its own fp32 accumulation error straddles a rounding boundary; with `carry`, also
+    what dx moves the pre-activation by) and, for a ReLU, the rows whose mask the accumulation error together with dx
+    leaves undetermined"""
     Wa = W.abs()
     y = x @ W.t()
     e_own = ACC32 * (x.abs() @ Wa.t())
     a, d, amb_own = _rounded(y, e_own, relu)
-    amb = _rounded(y, e_own + dx @ Wa.t(), True)[2] if relu else None
+    if relu or carry:
+        _, d_all, amb = _rounded(y, e_own + dx @ Wa.t(), relu)
+        if carry:
+            d = d_all
     return a, d, (amb, amb_own) if relu else None
 
 
@@ -117,6 +126,62 @@ def _wgrad(dO, dO_err, dO_abs, In, In_err, scale):
     return v, A, err
 
 
+def rgb_forward(rin, d_rin, rgb_params, rgb_act=1, carry=False):
+    """the rgb net 32 -> 64 -> 64 -> 3 from fp16 inputs rin (n, 32) the kernel may hold differently by up to d_rin, at the
+    kernel's rounding points (see mlp_forward for the dict it returns; k_mlp_rgb_fwd runs this alone)"""
+    dt = torch.float64
+    Wr = rgb_params.to(dt)
+    W1r, W2r, W3r = Wr[:2048].view(64, 32), Wr[2048:6144].view(64, 64), Wr[6144:7168].view(16, 64)
+    rin, d_rin = rin.to(dt), d_rin.to(dt)
+    r1, d_r1, amb_r1 = _fwd(rin, d_rin, W1r, True, carry)
+    r2, d_r2, amb_r2 = _fwd(r1, d_r1, W2r, True, carry)
+    W3 = W3r[:3]
+    yo = r2 @ W3.t()
+    eo = ACC32 * (r2.abs() @ W3.abs().t()) + d_r2 @ W3.abs().t()
+    f = dict(rin=rin, d_rin=d_rin, r1=r1, d_r1=d_r1, r2=r2, d_r2=d_r2, yo=yo, d_yo=eo,
+             ambiguous=amb_r1[0] | amb_r2[0], ambiguous_own=amb_r1[1] | amb_r2[1])
+    if rgb_act == 1:
+        # the kernel's fp32 sigmoid of its accumulator, within SIG_ERR of the sigmoid of a value in yo +- eo, then rounded
+        # to fp16: both steps are monotone, so its output lies between the roundings of the two ends
+        def sgm(v): return torch.sigmoid(v)
+        o = f16(sgm(yo))
+        s = o * (1 - o)
+        o_lo, o_hi = f16(sgm(yo - eo) - SIG_ERR), f16(sgm(yo + eo) + SIG_ERR)
+        ds = torch.maximum((o_lo * (1 - o_lo) - s).abs(), (o_hi * (1 - o_hi) - s).abs())
+        f.update(out=o, d_out=torch.maximum(o_hi - o, o - o_lo), s=s, d_s=ds)
+    else:
+        o, d_o, _ = _rounded(yo, eo, False)
+        f.update(out=o, d_out=d_o)
+    return f
+
+
+def mlp_forward(feat, sh, enc_mlp, rgb_params, rgb_act=1, carry=False, d_feat=None):
+    """the network forward from fp16 features at the kernel's rounding points, as intervals (k_ngp_fwd's MLP part, and
+    what k_ngp_bwd3 recomputes). feat (n, 32) fp16 features, sh (n, 16) float64 SH-4 (unrounded), enc_mlp (>= 3072) /
+    rgb_params (7168) fp16 weights. Returns a dict of float64 tensors:
+      hid, h, rin = [fp16(sh) | h], r1, r2: fp16 values, each with d_<name>, how far the kernel's value may be from it;
+      yo (n, 3): the rgb net's pre-activation, d_yo its bound (fp32 accumulation plus what d_r2 moves);
+      out (n, 3): the rgb output, an fp16 value (half_round), d_out its bound; for rgb_act 1 also s = out (1 - out)
+      and d_s, what the sigmoid derivative of the kernel's output may differ by;
+      ambiguous / ambiguous_own (n) bool: rows whose ReLU masks are undetermined (module docstring).
+    carry=False is the backward's model: d_<name> is one flip of the value's own rounding, and a flip reaches only the
+    next layer's masks. carry=True bounds the forward's outputs: every layer's bound also carries what its inputs'
+    bounds move it by, so a value rounded the other way is followed to the outputs. d_feat: how far the kernel's
+    features may lie from feat (grid_encode's bound); None when feat are the kernel's own (feat_save)."""
+    dt = torch.float64
+    feat = feat.to(dt)
+    d_feat = torch.zeros_like(feat) if d_feat is None else d_feat.to(dt)
+    Wd = enc_mlp.to(dt)
+    W1d, W2d = Wd[:2048].view(64, 32), Wd[2048:3072].view(16, 64)
+    hid, d_hid, amb_hid = _fwd(feat, d_feat, W1d, True, carry)
+    h, d_h, _ = _fwd(hid, d_hid, W2d, False, carry)
+    shr, d_sh, _ = _rounded(sh.to(dt), SH_ERR, False)
+    f = rgb_forward(torch.cat([shr, h], 1), torch.cat([d_sh, d_h], 1), rgb_params, rgb_act, carry)
+    f.update(hid=hid, d_hid=d_hid, h=h, d_h=d_h, ambiguous=amb_hid[0] | f["ambiguous"],
+             ambiguous_own=amb_hid[1] | f["ambiguous_own"])
+    return f
+
+
 def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1):
     """feat (n, 32) fp16 features, sh (n, 16) float64 SH-4 (unrounded), enc_mlp (>= 3072) / rgb_params (7168) fp16 weights,
     up_sig (n), up_rgb (n, 3) fp32 upstream gradients, scale the power-of-two loss scale (a number).
@@ -131,22 +196,11 @@ def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1
     up_sig, up_rgb = up_sig.to(dt), up_rgb.to(dt)
 
     # ---- forward recompute with the kernel's rounding points, as intervals ----
-    zero = torch.zeros_like(feat)
-    hid, d_hid, amb_hid = _fwd(feat, zero, W1d, True)
-    h, d_h, _ = _fwd(hid, d_hid, W2d, False)
-    shr, d_sh, _ = _rounded(sh.to(dt), SH_ERR, False)
-    rin, d_rin = torch.cat([shr, h], 1), torch.cat([d_sh, d_h], 1)
-    r1, d_r1, amb_r1 = _fwd(rin, d_rin, W1r, True)
-    r2, d_r2, amb_r2 = _fwd(r1, d_r1, W2r, True)
-    W3 = W3r[:3]
-    yo = r2 @ W3.t()
-    eo = ACC32 * (r2.abs() @ W3.abs().t()) + d_r2 @ W3.abs().t()
+    f = mlp_forward(feat, sh, enc_mlp, rgb_params, rgb_act)
+    hid, d_hid, h, d_h, rin, d_rin = f["hid"], f["d_hid"], f["h"], f["d_h"], f["rin"], f["d_rin"]
+    r1, d_r1, r2, d_r2, yo = f["r1"], f["d_r1"], f["r2"], f["d_r2"], f["yo"]
     if rgb_act == 1:
-        def sgm(v): return torch.sigmoid(v)
-        o = f16(sgm(yo))
-        s = o * (1 - o)
-        o_lo, o_hi = f16(sgm(yo - eo) - SIG_ERR), f16(sgm(yo + eo) + SIG_ERR)
-        ds = torch.maximum((o_lo * (1 - o_lo) - s).abs(), (o_hi * (1 - o_hi) - s).abs())
+        o, s, ds = f["out"], f["s"], f["d_s"]
     else:
         s, ds = torch.ones_like(yo), torch.zeros_like(yo)
 
@@ -181,7 +235,7 @@ def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1
         "W1d": _wgrad(dhid, dhid_err, dhid_abs, feat, torch.zeros_like(feat), scale),
     }
     return dict(dfeat=dfeat, dfeat_err=dfeat_err, dfeat_abs=dfeat_abs, dW=dW,
-                ambiguous=amb_hid[0] | amb_r1[0] | amb_r2[0], ambiguous_own=amb_hid[1] | amb_r1[1] | amb_r2[1],
+                ambiguous=f["ambiguous"], ambiguous_own=f["ambiguous_own"],
                 hid=hid, h=h, rin=rin, r1=r1, r2=r2, o=o if rgb_act == 1 else yo,
                 chain=[dout, dr2, dr1, dh, dhid, dfeat])
 
@@ -195,6 +249,82 @@ def split_dW(grad_enc, grad_rgb):
     """the five weight gradients of flat gradient vectors, as (out, in) matrices"""
     src = {"enc": grad_enc, "rgb": grad_rgb}
     return {k: src[v][o:o + s[0] * s[1]].view(*s) for k, (v, o, s) in DW_LAYOUT.items()}
+
+
+# ---------------------------------------------------------------------------------------------------
+# network forward: the features, sigma, the stand-alone SH encoding and the ray-mode positions
+# ---------------------------------------------------------------------------------------------------
+EXP_ERR = 2.0 ** -22   # relative error of expf (2 ulp: CUDA C++ Programming Guide; the build does not use fast-math)
+FMA_CHAIN = 8 * 2.0 ** -24  # grid_lookup's 8-step fmaf chain: one fp32 rounding a step, each <= 2^-24 sum |w_k t_k|
+
+
+def grid_encode(meta, table_h, x01):
+    """encode_rows (grid_lookup, then pack_half2) as intervals. table_h (entries, 2) fp16 table, x01 (n, 3) float32.
+    Returns float64 (n, 32) tensors: feat = fp16 of the float64 sum_k w_k t_k (column 2 l + f; levels >= n_levels are
+    exactly 0) and d_feat, how far the kernel's fp16 value may lie from it. The weights and indices are the kernel's bit
+    for bit (corner_weights, corner_indices: the dense wrap and the clamp outside the box included), so the products
+    w_k t_k (24 x 11 bits) are exact and only the fp32 chain and the fp16 rounding are left."""
+    n = x01.shape[0]
+    feat = torch.zeros(n, 32, dtype=torch.float64, device=x01.device)
+    d_feat = torch.zeros_like(feat)
+    t = table_h.double()
+    for l in range(int(meta.n_levels)):
+        off = int(meta.offset[l])
+        entries = int(meta.offset[l + 1]) - off
+        w, gi = corner_weights(x01, meta.scale[l])
+        idx = corner_indices(gi, int(meta.res[l]), entries, bool((int(meta.hashed_mask) >> l) & 1)) + off
+        c = w.double()[:, :, None] * t[idx]
+        a, d, _ = _rounded(c.sum(1), FMA_CHAIN * c.abs().sum(1), False)
+        feat[:, 2 * l:2 * l + 2], d_feat[:, 2 * l:2 * l + 2] = a, d
+    return feat, d_feat
+
+
+def sigma(h, d_h):
+    """sigma = expf(h0) of the kernel's fp16 h0, which lies in h[:, 0] +- d_h[:, 0]: (float64 exp(h0), bound)"""
+    h0, d0 = h[:, 0], d_h[:, 0]
+    s = torch.exp(h0)
+    lo, hi = torch.exp(h0 - d0), torch.exp(h0 + d0)
+    return s, torch.maximum(hi - s, s - lo) + EXP_ERR * hi + 2.0 ** -148  # + two fp32 subnormal steps
+
+
+def sh_encode(u):
+    """k_sh_encode: SH-4 of fmaf(u, 2, -1) (one float32 rounding of the exact 2u - 1), in float64, then rounded to fp16
+    as intervals: (value, bound). For u in [0, 1]^3 the kernel's fp32 SH is within SH_ERR of the float64 one."""
+    from .oracle import torch_sh4
+    x = (u.double() * 2 - 1).float().double()
+    a, d, _ = _rounded(torch_sh4(x), SH_ERR, False)
+    return a, d
+
+
+def ray_positions(rays_o, rays_d, ray_idx, ts):
+    """load_sample's ray-mode position x = fma(d, t, o) in float32, bit for bit; (n, 3), 0 where ray_idx < 0.
+    The float64 product d t is exact; the float64 sum s = d t + o is rounded at most once and TwoSum gives its exact
+    residual r. Rounding s to float32 gives the fma's result unless s is exactly halfway between two floats while
+    r != 0 -- then the fma rounds towards r."""
+    live = ray_idx >= 0
+    r = ray_idx.long().clamp_min(0)
+    p = rays_d[r].double() * ts.double()[:, None]
+    o = rays_o[r].double()
+    s = p + o
+    bp = s - o
+    res = (p - bp) + (o - (s - bp))
+    x = s.float()
+    xd = x.double()
+    nb = torch.where(s > xd, torch.nextafter(x, torch.full_like(x, float("inf"))),
+                     torch.nextafter(x, torch.full_like(x, -float("inf"))))
+    tie = (s != xd) & ((s - xd) == (nb.double() - s)) & (res != 0)
+    x = torch.where(tie & (res > 0), torch.maximum(x, nb), torch.where(tie & (res < 0), torch.minimum(x, nb), x))
+    return torch.where(live[:, None], x, torch.zeros_like(x))
+
+
+def to_unit(x, xyz_min, xyz_max):
+    """to_unit: __fdiv_rn(x - xyz_min, xyz_max - xyz_min) in float32, bit for bit (a float32 difference and quotient are
+    exact in float64 -- 53 >= 2 x 24 + 2 -- so one rounding to float32 each is the kernel's)"""
+    mn = torch.tensor(xyz_min, dtype=torch.float64, device=x.device)
+    mx = torch.tensor(xyz_max, dtype=torch.float64, device=x.device)
+    num = (x.double() - mn).float().double()
+    den = (mx - mn).float().double()
+    return (num / den).float()
 
 
 # ---------------------------------------------------------------------------------------------------

@@ -261,7 +261,7 @@ def _train_and_score(bank, test, strategy, steps=1000, seed=0):
 def test_nerf_fixture_trains_like_the_in_memory_bank(tmp_path):
     """SynthLego written as a NeRF-synthetic scene (RGBA PNGs, Blender axes, radius 4) and loaded back trains to the test
     PSNR of the same run on synth.RayBank -- same resolution, steps, seed and sampling strategy, hence the same (image,
-    pixel) draws -- within 0.5 dB (means over two seeds), under both strategies. (At 1000 steps 'same_image' itself scores
+    pixel) draws -- within 0.5 dB (means over six seeds), under both strategies. (At 1000 steps 'same_image' itself scores
     ~0.9 dB below 'all_images' on this scene: one image per batch gives correlated gradients.)"""
     import dataset_fixtures as F
     from ngp_pl_b200 import datasets, synth
@@ -275,10 +275,14 @@ def test_nerf_fixture_trains_like_the_in_memory_bank(tmp_path):
     # fixture and the GPU trace of the bank round differently
     assert (bank.poses - train.poses).abs().max() < 1e-6
     assert ((bank.rgb.float() / 255 - train.rgb).abs().max(-1)[0] > 1e-6).float().mean() < 0.01
-    # mean over two seeds: one 'same_image' run moves by ~0.8 dB when the bank's edge pixels change in the last bit
+    # Training is not bitwise repeatable (the table gradients are fp32 atomics), and 'same_image' amplifies that: two runs
+    # of the same seed on the same bank differed by up to 1.3 dB (seed 0; seeds 1-7 by <= 0.35 dB; 'all_images' by
+    # <= 0.12 dB; H100 80GB HBM3, 700 W). A mean over two seeds then moves by 0.6 dB from run to run; over six, one such
+    # seed moves it by <= 0.22 dB
+    seeds = range(6)
     for s in ("all_images", "same_image"):
-        base = np.mean([_train_and_score(bank, test, s, seed=k) for k in (0, 1)])
-        got = np.mean([_train_and_score(train, test, s, seed=k) for k in (0, 1)])
+        base = np.mean([_train_and_score(bank, test, s, seed=k) for k in seeds])
+        got = np.mean([_train_and_score(train, test, s, seed=k) for k in seeds])
         print("%s test PSNR: RayBank %.3f, load_scene %.3f" % (s, base, got))
         assert base > 24 and abs(got - base) < 0.5, (s, got, base)
 

@@ -2,13 +2,19 @@
 silently agree with a wrong kernel (tests/test_backward_fp64_gpu.py compares the kernels with it):
   * its network backward against fp32 autograd of oracle.torch_ngp_forward (rgb_act 0 and 1);
   * its table scatter against float64 autograd of oracle.torch_grid_encode (dense, hashed and wrapping corners);
-  * its feat_save decoder against a plain encoder of the documented fragment layout.
+  * its feat_save decoder against a plain encoder of the documented fragment layout;
+  * mlp_backward against its own stored outputs (tests/golden/grad64_mlp_backward.npz), so that a change to the forward
+    it shares with mlp_forward shows.
 """
+import os
+
 import numpy as np
 import pytest
 import torch
 
 from oracle import grad64
+
+GOLDEN_MLP = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "grad64_mlp_backward.npz")
 
 
 def _points(n, seed, lo=-0.5, hi=0.5):
@@ -130,3 +136,130 @@ def test_feat_save_decoder_vs_fragment_layout():
     raw.reshape(2, 2, 32, 4, 2)[0, 0, 4 * 3 + 1, 1, 0] = 1.0  # tile 0, kt 0, g = 3, q = 1, word y (row g + 8), low half
     dec = grad64.decode_feat_save(torch.as_tensor(raw.view(np.uint8)), 16)
     assert dec[11, 2].item() == 1.0 and dec.abs().sum().item() == 1.0
+
+
+def mlp_backward_outputs():
+    """mlp_backward on one seeded batch of fp16 features (rgb_act 1 and 0): every output as a named float64 / bool array.
+    The weight gradients are kept for rgb_act 1 only (they are most of the bytes)."""
+    enc, rgb = _params(0, 13)
+    g = torch.Generator().manual_seed(14)
+    n = 48
+    feat = (torch.rand(n, 32, generator=g) * 2 - 1).half()
+    d = torch.randn(n, 3, generator=g, dtype=torch.float64)
+    up_sig = torch.randn(n, generator=g) * 1e-2
+    up_rgb = torch.randn(n, 3, generator=g) * 1e-1
+    out = {}
+    for act in (1, 0):
+        ref = grad64.mlp_backward(feat, grad64.sh4_64(d), enc[:3072].half(), rgb.half(), up_sig, up_rgb, 2.0 ** 10, act)
+        keys = ["dfeat", "dfeat_err", "dfeat_abs", "ambiguous", "ambiguous_own", "hid", "h", "rin", "r1", "r2", "o"]
+        for k in keys:
+            out["act%d_%s" % (act, k)] = ref[k].numpy()
+        for i, c in enumerate(ref["chain"]):
+            out["act%d_chain%d" % (act, i)] = c.numpy()
+        if act == 1:
+            for k, (v, A, err) in ref["dW"].items():
+                out["act1_dW_%s_v" % k], out["act1_dW_%s_A" % k], out["act1_dW_%s_err" % k] = v.numpy(), A.numpy(), err.numpy()
+    return out
+
+
+def test_mlp_backward_unchanged():
+    """mlp_backward gives what it gave before its forward recompute became mlp_forward. Bounds and masks must not move;
+    2^-40 relative leaves room only for another float64 summation order in the matrix products."""
+    want = np.load(GOLDEN_MLP)
+    got = mlp_backward_outputs()
+    assert sorted(got) == sorted(want.files)
+    for k in want.files:
+        a, b = got[k], want[k]
+        assert a.shape == b.shape and a.dtype == b.dtype, k
+        if a.dtype == np.bool_:
+            assert (a == b).all(), k
+        else:
+            assert (np.abs(a - b) <= 2.0 ** -40 * np.abs(b).max()).all(), k
+
+
+def _within(got, want, bound, keep, what):
+    """|got - want| <= 2 bound on the rows in keep; returns the worst ratio |got - want| / (2 bound) there"""
+    got, want, bound = got.double(), want.double(), bound.double()
+    if got.dim() == 1:
+        got, want, bound = got[:, None], want[:, None], bound[:, None]
+    err = (got - want).abs()[keep]
+    b = 2 * bound[keep]
+    bad = err > b
+    assert not bad.any(), "%s: %d values outside 2 x bound, worst excess %g" % (what, int(bad.sum()), float((err - b).max()))
+    return float((err / b.clamp_min(1e-300)).max())
+
+
+@pytest.mark.parametrize("cfg", [(16, 19, 1), (4, 14, 1), (16, 19, 0)])
+def test_interval_forward_contains_the_fp32_oracles(oracle, cfg):
+    """grid_encode, mlp_forward(carry=True) and sigma contain the fp32 outputs of oracle.torch_ngp_forward and of the C
+    oracle: both take the kernel's fp16 rounding points, so they differ from the float64 values only by fp32 arithmetic"""
+    L, log2_T, act = cfg
+    meta, total = oracle.grid_meta(L, log2_T, 16, float(np.float32(np.exp(np.log(2048 * 0.5 / 16) / (L - 1)))))
+    enc, rgb = _params(total, 21)
+    n = 300
+    x, d = _points(n, 22)
+    x[:4] = torch.tensor([[-0.5, -0.5, -0.5], [0.5, 0.5, 0.5], [0.5, -0.5, 0.0], [0.0, 0.0, 0.0]])
+    d[4:8] *= torch.tensor([[1e-6], [1e-3], [1e3], [1e6]])
+    mn, mx = torch.full((1, 3), -0.5), torch.full((1, 3), 0.5)
+    x01 = grad64.to_unit(x, [-0.5] * 3, [0.5] * 3)
+    assert torch.equal(x01, (x - mn) / (mx - mn))
+    feat, d_feat = grad64.grid_encode(meta, enc[3072:].half().view(-1, 2), x01)
+    f = grad64.mlp_forward(feat, grad64.sh4_64(d), enc[:3072].half(), rgb.half(), act, carry=True, d_feat=d_feat)
+    sig, d_sig = grad64.sigma(f["h"], f["d_h"])
+    # no row is left out: a carried bound holds through a ReLU whose mask it leaves open (relu and the fp16 rounding are
+    # monotone, so the kernel's value lies between the roundings of the interval's ends)
+    keep = torch.ones(n, dtype=torch.bool)
+    with torch.no_grad():
+        ft = oracle.torch_grid_encode(meta, enc[3072:].view(-1, 2), x01)
+        sig_t, rgb_t, h_t = oracle.torch_ngp_forward(meta, enc, rgb, mn, mx, x, d, rgb_act=act)
+    sig_c, rgb_c, h_c = oracle.ngp_forward_c(meta, enc.numpy(), rgb.numpy(), mn.numpy(), mx.numpy(), x.numpy(), d.numpy(),
+                                             rgb_act=act)
+    _within(ft, feat, d_feat, keep, "torch features")
+    assert (feat[:, 2 * L:] == 0).all() and (d_feat[:, 2 * L:] == 0).all()
+    for name, (s_, r_, h_) in {"torch": (sig_t, rgb_t, h_t), "C": tuple(map(torch.as_tensor, (sig_c, rgb_c, h_c)))}.items():
+        _within(h_, f["h"], f["d_h"], keep, name + " h")
+        _within(s_, sig, d_sig, keep, name + " sigma")
+        _within(r_, f["out"], f["d_out"], keep, name + " rgb")
+    # the bounds stay tight: most feature bounds are zero (no rounding boundary within reach of the fp32 chain), and the
+    # sigmoid's outputs are bounded to a few fp16 ulps even with every feature's possible flip carried through the net
+    assert (d_feat == 0).double().mean() > 0.9
+    if act == 1:
+        assert (f["d_out"] <= 16 * 2.0 ** -11).all()
+
+
+def test_sh_encode_and_ray_positions_restatements():
+    """sh_encode against the fp32 SH of fmaf(u, 2, -1) rounded to fp16; ray_positions bit for bit against float32 fma,
+    including sums that the float64 addition rounds onto a float32 halfway point"""
+    from oracle.oracle import torch_sh4
+    rng = np.random.RandomState(31)
+    u = torch.as_tensor(rng.uniform(0, 1, (500, 3)).astype(np.float32))
+    u[:3] = torch.tensor([[0, 0, 0], [1, 1, 1], [0.5, 0.25, 0.75]])
+    v, dv = grad64.sh_encode(u)
+    got = torch_sh4(torch.addcmul(torch.full_like(u, -1.0), u, torch.full_like(u, 2.0))).half().double()
+    _within(got, v, dv, torch.ones(500, dtype=torch.bool), "sh")
+    # fma(d, t, o) in float32: np.float32 has no fma, so take the correctly rounded exact value from Python fractions
+    from fractions import Fraction
+    o = rng.uniform(-1, 1, (40, 3)).astype(np.float32)
+    dr = rng.normal(size=(40, 3)).astype(np.float32)
+    ridx = rng.randint(-1, 40, 300).astype(np.int32)
+    ts = rng.uniform(0, 3, 300).astype(np.float32)
+    # halfway cases: o = 1, d t = 2^-24 + 2^-60 -> the float64 sum is 1 + 2^-24 exactly (a float32 tie), the fma rounds up
+    o[0] = [1.0, 1.0, -1.0]
+    dr[0] = [2.0 ** -24 + 2.0 ** -47, -(2.0 ** -24 + 2.0 ** -47), 2.0 ** -25 + 2.0 ** -48]
+    ridx[:4] = 0
+    ts[:4] = np.float32(1 + 2.0 ** -13)
+    x = grad64.ray_positions(torch.as_tensor(o), torch.as_tensor(dr), torch.as_tensor(ridx), torch.as_tensor(ts)).numpy()
+    for i in range(300):
+        r = ridx[i]
+        for k in range(3):
+            if r < 0:
+                assert x[i, k] == 0
+                continue
+            exact = Fraction(float(dr[r, k])) * Fraction(float(ts[i])) + Fraction(float(o[r, k]))
+            lo = np.float32(float(exact))  # nearest double, then the float32 neighbours around it
+            cands = [np.nextafter(lo, np.float32(-np.inf)), lo, np.nextafter(lo, np.float32(np.inf))]
+            dist = [abs(Fraction(float(c)) - exact) for c in cands]
+            best = min(dist)
+            ties = [c for c, e in zip(cands, dist) if e == best]
+            want = ties[0] if len(ties) == 1 else [c for c in ties if not (c.view(np.int32) & 1)][0]
+            assert x[i, k] == want, (i, k, float(x[i, k]), float(want))

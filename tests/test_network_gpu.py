@@ -4,8 +4,8 @@ C restatement oracle_ngp_forward).
 
 tinycudann is absent from /root/reference, so this part of the path is "parity unpinned" against the
 reference; what is pinned here is the CUDA kernel against the restated algorithm:
-  features / h / rgb : fp16-level error (a few fp16 ulps; accumulation order differs)
-  sigmas             : exp of an fp16 value -> same relative error as h0's absolute error
+  level table        : equal to the oracle's; the forward's outputs are held per sample to the float64 bounds of
+                       oracle/grad64.py by tests/test_forward_fp64_gpu.py
   gradients          : compared with autograd of the oracle, normalised by the gradient's max
 """
 import ctypes as C
@@ -66,15 +66,9 @@ def test_forward_vs_oracle(cfg, oracle):
     xyz_max = torch.full((1, 3), scale)
     sig_o, rgb_o, h_o = oracle.torch_ngp_forward(meta_o, enc, rgbp, xyz_min, xyz_max, torch.as_tensor(x), torch.as_tensor(d))
     sig_c, rgb_c, h_c = oracle.ngp_forward_c(meta_o, enc.numpy(), rgbp.numpy(), xyz_min.numpy(), xyz_max.numpy(), x, d)
-    # the two oracle restatements agree with each other (C fmaf chain vs torch matmul: fp16-ulp level)
+    # the two oracle restatements agree with each other (C fmaf chain vs torch matmul: fp16-ulp level); the kernel's
+    # sigma and rgb are checked per sample against float64 bounds in tests/test_forward_fp64_gpu.py
     assert np.abs(h_c - h_o.numpy()).max() < 0.02 * max(1.0, np.abs(h_c).max())
-    h_scale = max(1.0, float(h_o.abs().max()))
-    err_sig = (torch.log(sig.cpu()) - torch.log(sig_o)).abs().max().item()
-    assert err_sig < 0.01 * h_scale, "log-sigma error %g" % err_sig
-    err_rgb = (rgb.cpu() - rgb_o).abs().max().item()
-    assert err_rgb < 4e-3, "rgb error %g" % err_rgb
-    # typical (median) error is far below the fp16 rounding-flip outliers
-    assert (rgb.cpu() - rgb_o).abs().median().item() < 5e-4
 
 
 def test_backward_vs_oracle_autograd(oracle):
