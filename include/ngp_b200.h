@@ -183,7 +183,10 @@ int ngp_net_backward(const NgpNet* net, const NgpSamples* smp, const float* dL_d
                      const void* feat_save, const float* loss_scale, float* grad_enc, float* grad_rgb,
                      void* workspace, size_t workspace_bytes, void* stream);
 
-/* The two halves of ngp_net_backward, individually callable (profiling; overlapping them with other work). */
+/* The two halves of ngp_net_backward, individually callable (profiling; overlapping them with other work).
+ * Both launch as programmatic dependents of the kernel before them on the stream (they may start under its tail):
+ * the MLP half reads the fp16 weights, and the scatter half the sample count, live list and sample positions, before
+ * waiting for that kernel, so these must not be written by the kernel issued immediately before the call. */
 int ngp_net_backward_mlp(const NgpNet* net, const NgpSamples* smp, const float* dL_dsigmas, const float* dL_drgbs,
                          const void* feat_save, const float* loss_scale, float* grad_enc, float* grad_rgb,
                          void* workspace, size_t workspace_bytes, void* stream);
@@ -303,7 +306,9 @@ int ngp_nerf_loss_grad(const NgpTrainCfg* cfg, const NgpTrainBuffers* buf, const
  * g = grads * grad_mul (1/world_size after a sum all-reduce). Also refreshes the fp16 working copy and
  * zeroes the gradient for the next step in the same pass. lr and step live on the device
  * (lr_dev[0], step_dev[0] = number of completed steps; the kernel uses t = step+1 and a follow-up
- * single-thread kernel increments it) so a captured CUDA graph never needs re-capturing. */
+ * single-thread kernel increments it) so a captured CUDA graph never needs re-capturing. Launched as a programmatic
+ * dependent of the kernel before it on the stream: params, exp_avg, exp_avg_sq, lr and step are read before waiting
+ * for that kernel, so they must not be written by the kernel issued immediately before the call. */
 int ngp_adam_step(float* params, float* grads, float* exp_avg, float* exp_avg_sq, uint16_t* params_half, int64_t n,
                   const float* lr_dev, int32_t* step_dev, float beta1, float beta2, float eps, float grad_mul,
                   int increment_step, void* stream);

@@ -49,6 +49,36 @@ __device__ __forceinline__ void trace_mark(unsigned long long* buf, int id) {  /
 
 static inline int ngp_div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// Programmatic dependent launch (sm_90). The training step is a serial chain of kernels on one stream; launched with
+// ngp_launch_pdl(), a kernel may start while its immediate predecessor in the stream is still running (stream capture
+// records the edge as a programmatic graph edge), so its launch latency and prologue hide under the predecessor's tail.
+// pdl_wait() returns once the predecessor has completed and its writes are visible; pdl_trigger() lets the successor
+// launch. A kernel launched without the attribute (any plain <<<>>> launch) returns from pdl_wait() at once.
+// The rules that make a chain of such kernels safe:
+//  - every thread of a kernel calls pdl_wait() exactly once, before it exits, and pdl_trigger() only after its own
+//    pdl_wait(). Then, when a kernel starts, every kernel before its immediate predecessor has completed and its writes
+//    are visible;
+//  - before its pdl_wait(), a kernel reads nothing its immediate predecessor writes;
+//  - before its pdl_wait(), a kernel writes nothing its immediate predecessor reads or writes.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+template <typename... KArgs, typename... Args>
+static inline cudaError_t ngp_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                         Args&&... args) {
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
 // Number of SMs of the current device (132 on H100 SXM); cached per process.
 static inline int ngp_sm_count() {
     static int sms = 0;

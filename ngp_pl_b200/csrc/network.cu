@@ -239,6 +239,9 @@ __global__ void __launch_bounds__(FWD_THREADS, FWD_MIN_BLOCKS)
 k_ngp_fwd(const NgpNet net, const NgpSamples smp, const int want_rgb, float* __restrict__ sigmas, float* __restrict__ rgbs,
           __half* __restrict__ h_out, uint4* __restrict__ feat_save, int* __restrict__ sched) {
     __shared__ __align__(16) MlpWeightsFwd sw;
+    // (eager callers may write the weights or the samples with the kernel right before this one: wait first)
+    pdl_wait();
+    pdl_trigger();
     const __half* wd = reinterpret_cast<const __half*>(net.enc_params_h);
     const __half* wr = want_rgb ? reinterpret_cast<const __half*>(net.rgb_params_h) : nullptr;
     load_weights_fwd(sw, wd, wr, threadIdx.x, FWD_THREADS);
@@ -369,8 +372,8 @@ extern "C" int ngp_net_forward(const NgpNet* net, const NgpSamples* smp, int wan
     const int64_t want = (n_tiles + FWD_THREADS / 32 - 1) / (FWD_THREADS / 32);
     const int64_t cap = (int64_t)ngp_sm_count() * FWD_MIN_BLOCKS;
     const int grid = (int)(want < cap ? want : cap);
-    k_ngp_fwd<<<grid, FWD_THREADS, 0, st>>>(*net, *smp, want_rgb, sigmas, rgbs, (__half*)h_out, (uint4*)feat_save,
-                                            sched_slot(st));
+    NGP_CUDA(ngp_launch_pdl(k_ngp_fwd, grid, FWD_THREADS, 0, st, *net, *smp, want_rgb, sigmas, rgbs, (__half*)h_out,
+                            (uint4*)feat_save, sched_slot(st)));
     NGP_CHECK_LAUNCH();
     NGP_TRACE(3, st);
     return 0;
@@ -551,16 +554,14 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
     Bwd3Smem& S = *reinterpret_cast<Bwd3Smem*>(smem_raw);
     const __half* wd = reinterpret_cast<const __half*>(net.enc_params_h);
     const __half* wr = reinterpret_cast<const __half*>(net.rgb_params_h);
+    // Before waiting on the kernel that publishes the live count and the loss scale: stage the weights (the fp16 working
+    // copy, written by the previous step's optimiser), initialise the barriers and take the first ticket (the scheduler
+    // slot is this launch's own).
     load_weights_fwd(S.wf, wd, wr, threadIdx.x, B3_THREADS);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
     const bool mma_wg = warp >= B3_WARPS;
-    const int64_t n = bwd_count(smp);
     const int32_t* __restrict__ live = smp.live_idx;
-    const int64_t n_mtiles = (n + 15) / 16;
-    const int64_t n_blks = (n_mtiles + B3_WARPS - 1) / B3_WARPS;
-    const float scale = loss_scale ? *loss_scale : 1.0f;
-    const float inv_scale = 1.0f / scale;
     const int row0 = 16 * warp;
 
     if (threadIdx.x == 0) {
@@ -571,6 +572,13 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         S.blk[0] = sched ? atomicAdd(&sched[0], 1) : (int)blockIdx.x;
     }
+    pdl_wait();
+    pdl_trigger();
+    const int64_t n = bwd_count(smp);
+    const int64_t n_mtiles = (n + 15) / 16;
+    const int64_t n_blks = (n_mtiles + B3_WARPS - 1) / B3_WARPS;
+    const float scale = loss_scale ? *loss_scale : 1.0f;
+    const float inv_scale = 1.0f / scale;
     __syncthreads();
     uint32_t commits[2] = {0u, 0u};  // MMA batches signalled on done[b] so far (every thread counts the same)
 
@@ -896,17 +904,26 @@ k_grid_scatter_merged(const NgpNet net, const NgpSamples smp, const uint32_t* __
                       const float* __restrict__ loss_scale, float* __restrict__ grad_table) {
     const int lane = threadIdx.x & 31;
     const int64_t n = bwd_count(smp);
-    const float inv_scale = loss_scale ? 1.0f / *loss_scale : 1.0f;
     const int64_t n_pad = (n + 31) & ~(int64_t)31;
     const int n_levels = net.meta.n_levels;
 
-    for (int64_t s = blockIdx.x * (int64_t)SCATTER_THREADS + threadIdx.x; s < n_pad; s += (int64_t)gridDim.x * SCATTER_THREADS) {
-        bool valid = s < n;
-        // the sample position is computed once and reused for all levels (dfeat is indexed by s, the position by
-        // the sample it stands for)
+    // the sample position is computed once and reused for all levels (dfeat is indexed by s, the position by the sample
+    // it stands for)
+    bool valid;
+    float u, v, w;
+    auto position = [&](int64_t s) {
+        valid = s < n;
         const SampleIn sm = load_sample(smp, (valid && smp.live_idx) ? (int64_t)__ldg(smp.live_idx + s) : s, valid);
-        float u, v, w;
         to_unit(net, sm, u, v, w);
+    };
+    // this thread's first sample (the count, the live list and the positions were written two or more kernels earlier) is
+    // loaded before waiting on the MLP backward, whose feature gradients are the first thing read after it
+    int64_t s = blockIdx.x * (int64_t)SCATTER_THREADS + threadIdx.x;
+    position(s);
+    pdl_wait();
+    pdl_trigger();
+    const float inv_scale = loss_scale ? 1.0f / *loss_scale : 1.0f;
+    for (; s < n_pad; s += (int64_t)gridDim.x * SCATTER_THREADS, position(s)) {
         const unsigned vmask = __ballot_sync(0xffffffffu, valid);
         // the per-level feature gradient is the one load on the critical path of a level: fetch the NEXT level's while
         // this level's shuffles and reductions run
@@ -1008,9 +1025,9 @@ extern "C" int ngp_net_backward_mlp(const NgpNet* net, const NgpSamples* smp, co
     const int64_t n_blks = (n_mtiles + B3_WARPS - 1) / B3_WARPS;
     const int grid = (int)(n_blks < (int64_t)ngp_sm_count() ? n_blks : ngp_sm_count());
     auto* kernel = feat_save ? k_ngp_bwd3<false> : k_ngp_bwd3<true>;
-    kernel<<<grid, B3_THREADS, sizeof(Bwd3Smem) + 128, (cudaStream_t)stream>>>(
-        *net, *smp, dL_dsigmas, dL_drgbs, (const uint4*)feat_save, loss_scale, grad_enc, grad_rgb, (uint32_t*)workspace,
-        n_mtiles * 16, sched_slot((cudaStream_t)stream));
+    NGP_CUDA(ngp_launch_pdl(kernel, grid, B3_THREADS, sizeof(Bwd3Smem) + 128, (cudaStream_t)stream, *net, *smp, dL_dsigmas,
+                            dL_drgbs, (const uint4*)feat_save, loss_scale, grad_enc, grad_rgb, (uint32_t*)workspace,
+                            n_mtiles * 16, sched_slot((cudaStream_t)stream)));
     NGP_CHECK_LAUNCH();
     NGP_TRACE(6, (cudaStream_t)stream);
     return 0;
@@ -1027,8 +1044,8 @@ extern "C" int ngp_net_backward_scatter(const NgpNet* net, const NgpSamples* smp
     int64_t gx = (smp->n + SCATTER_THREADS - 1) / SCATTER_THREADS;
     const int64_t cap = (int64_t)ngp_sm_count() * 8;
     if (gx > cap) gx = cap;
-    k_grid_scatter_merged<<<(unsigned)gx, SCATTER_THREADS, 0, (cudaStream_t)stream>>>(
-        *net, *smp, (const uint32_t*)workspace, n_mtiles * 16, loss_scale, grad_enc + NGP_DENSITY_MLP_PARAMS);
+    NGP_CUDA(ngp_launch_pdl(k_grid_scatter_merged, (unsigned)gx, SCATTER_THREADS, 0, (cudaStream_t)stream, *net, *smp,
+                            (const uint32_t*)workspace, n_mtiles * 16, loss_scale, grad_enc + NGP_DENSITY_MLP_PARAMS));
     NGP_CHECK_LAUNCH();
     NGP_TRACE(7, (cudaStream_t)stream);
     return 0;

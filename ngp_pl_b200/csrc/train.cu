@@ -232,6 +232,8 @@ __global__ void k_train_composite_bw(const NgpTrainCfg cfg, const int* __restric
 }
 
 __global__ void k_train_grad_scale(float* __restrict__ scalars, int* __restrict__ counters, const int fused_loss) {
+    pdl_wait();
+    pdl_trigger();
     // the live list is complete: publish its length and re-arm the append counter, so that counters[4] is zero
     // whenever a compositing backward starts, whatever the caller's order of calls
     counters[5] = counters[4];
@@ -270,6 +272,8 @@ __global__ void __launch_bounds__(CL_WARPS * 32) k_train_composite_loss(const Ng
                                        float* __restrict__ depth, float* __restrict__ dsigmas, float* __restrict__ drgbs,
                                        float* __restrict__ scalars, int* __restrict__ live_idx, int* __restrict__ counters,
                                        const float* __restrict__ bg_dev) {
+    pdl_wait();
+    pdl_trigger();
     const float3 bg = batch_bg(cfg, bg_dev);
     const int lane = threadIdx.x & 31;
     // (n_rays is a multiple of the rays per block or the last block's spare warps idle on ray n_rays - 1 with n = 0 and
@@ -369,12 +373,13 @@ extern "C" int ngp_render_train_step(const NgpNet* net, const NgpTrainCfg* cfg, 
     NGP_TRACE(13, st);
     rc = ngp_net_forward(net, &smp, 1, b->sigmas, b->rgbs, nullptr, b->feat_save, stream);
     if (rc) return rc;
-    k_train_composite_loss<<<ngp_div_up(n, CL_WARPS), CL_WARPS * 32, 0, st>>>(
-        *cfg, b->n_samples, b->offsets, b->sigmas, b->rgbs, b->deltas, b->ts, rgb_gt, b->rgb, b->opacity, b->depth, b->dsigmas,
-        b->drgbs, b->scalars, b->live_idx, b->counters, b->bg_dev);
+    // the kernels of this chain are launched as programmatic dependents of their predecessor (common.cuh)
+    NGP_CUDA(ngp_launch_pdl(k_train_composite_loss, ngp_div_up(n, CL_WARPS), CL_WARPS * 32, 0, st, *cfg, b->n_samples,
+                            b->offsets, b->sigmas, b->rgbs, b->deltas, b->ts, rgb_gt, b->rgb, b->opacity, b->depth, b->dsigmas,
+                            b->drgbs, b->scalars, b->live_idx, b->counters, b->bg_dev));
     NGP_CHECK_LAUNCH();
     NGP_TRACE(4, st);
-    k_train_grad_scale<<<1, 1, 0, st>>>(b->scalars, b->counters, 1);
+    NGP_CUDA(ngp_launch_pdl(k_train_grad_scale, 1, 1, 0, st, b->scalars, b->counters, 1));
     NGP_CHECK_LAUNCH();
     NGP_TRACE(5, st);
     if (b->live_idx) {
@@ -398,7 +403,7 @@ extern "C" int ngp_render_train_bwd(const NgpNet* net, const NgpTrainCfg* cfg, c
         *cfg, b->n_samples, b->offsets, b->sigmas, b->rgbs, b->deltas, b->ts, b->ws, b->rgb, b->opacity, b->depth, dL_drgb,
         dL_dopacity, dL_ddepth, dL_dws, b->dsigmas, b->drgbs, b->scalars, b->live_idx, b->counters, b->bg_dev);
     NGP_CHECK_LAUNCH();
-    k_train_grad_scale<<<1, 1, 0, st>>>(b->scalars, b->counters, 0);
+    NGP_CUDA(ngp_launch_pdl(k_train_grad_scale, 1, 1, 0, st, b->scalars, b->counters, 0));
     NGP_CHECK_LAUNCH();
     NgpSamples smp = train_samples(cfg, b);
     if (b->live_idx && b->feat_save) {
@@ -468,6 +473,9 @@ __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __re
     const uint64_t stream_pol = l2_policy_evict_first(), keep_pol = l2_policy_evict_last();
     // two 64-byte groups per thread and trip: all eight 128-bit loads are issued before the first use, so the stream keeps
     // ~15 MB in flight even when the next step's march shares the SMs' issue slots
+    // The bias correction and the first trip's parameter and moment loads go ahead of waiting on the kernel that produces
+    // the gradients (the step counter, the learning rate, P, M and V are written by earlier steps only).
+    bool waited = false;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i0 = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i0 < n4; i0 += 2 * stride) {
         const int64_t i1 = i0 + stride;
@@ -478,11 +486,18 @@ __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __re
             const int64_t i = u ? i1 : i0;
             if (u == 0 || two) {
                 pv[u] = ld_f4_hint(reinterpret_cast<const float4*>(p) + i, stream_pol);
-                gv[u] = ld_f4_hint(reinterpret_cast<const float4*>(g) + i, stream_pol);
                 mv[u] = ld_f4_hint(reinterpret_cast<const float4*>(m) + i, stream_pol);
                 vv[u] = ld_f4_hint(reinterpret_cast<const float4*>(v) + i, stream_pol);
             }
         }
+        if (!waited) {
+            pdl_wait();
+            pdl_trigger();
+            waited = true;
+        }
+#pragma unroll
+        for (int u = 0; u < 2; ++u)
+            if (u == 0 || two) gv[u] = ld_f4_hint(reinterpret_cast<const float4*>(g) + (u ? i1 : i0), stream_pol);
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
             if (u == 1 && !two) break;
@@ -516,6 +531,10 @@ __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __re
             }
         }
     }
+    if (!waited) {
+        pdl_wait();
+        pdl_trigger();
+    }
     // tail
     for (int64_t i = (n4 << 2) + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const float gr = g[i] * grad_mul;
@@ -526,7 +545,16 @@ __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __re
         if (ph) ph[i] = __float2half_rn(p[i]);
     }
 }
-__global__ void k_step_inc(int* step) { *step += 1; }
+__global__ void k_step_inc(int* step) {
+    pdl_wait();
+    pdl_trigger();
+    *step += 1;
+}
+static int launch_step_inc(int* step_dev, cudaStream_t st) {
+    NGP_CUDA(ngp_launch_pdl(k_step_inc, 1, 1, 0, st, step_dev));
+    NGP_CHECK_LAUNCH();
+    return 0;
+}
 
 extern "C" int ngp_adam_step(float* params, float* grads, float* exp_avg, float* exp_avg_sq, uint16_t* params_half, int64_t n,
                              const float* lr_dev, int32_t* step_dev, float beta1, float beta2, float eps, float grad_mul,
@@ -542,15 +570,12 @@ extern "C" int ngp_adam_step(float* params, float* grads, float* exp_avg, float*
         const int cap = ngp_sm_count() * 2;
         if (grid > cap) grid = cap;
         NGP_TRACE(18, st);
-        k_adam<<<grid, 256, 0, st>>>(params, grads, exp_avg, exp_avg_sq, (__half*)params_half, n, lr_dev, step_dev, beta1,
-                                      beta2, eps, grad_mul);
+        NGP_CUDA(ngp_launch_pdl(k_adam, grid, 256, 0, st, params, grads, exp_avg, exp_avg_sq, (__half*)params_half, n, lr_dev,
+                                step_dev, beta1, beta2, eps, grad_mul));
         NGP_CHECK_LAUNCH();
         NGP_TRACE(8, st);
     }
-    if (increment_step) {
-        k_step_inc<<<1, 1, 0, st>>>(step_dev);
-        NGP_CHECK_LAUNCH();
-    }
+    if (increment_step) return launch_step_inc(step_dev, st);
     return 0;
 }
 
@@ -639,10 +664,7 @@ extern "C" int ngp_adam_step_p2p(int world, int rank, const uint64_t* peer_grads
                                           eps, 1.0f / (float)world);
         NGP_CHECK_LAUNCH();
     }
-    if (increment_step) {
-        k_step_inc<<<1, 1, 0, st>>>(step_dev);
-        NGP_CHECK_LAUNCH();
-    }
+    if (increment_step) return launch_step_inc(step_dev, st);
     return 0;
 }
 
@@ -892,10 +914,7 @@ extern "C" int ngp_adam_step_fused(int world, int rank, const uint64_t* peer_gra
 #undef NGP_LAUNCH_FUSED
     NGP_CHECK_LAUNCH();
     NGP_TRACE(8, st);
-    if (increment_step) {
-        k_step_inc<<<1, 1, 0, st>>>(step_dev);
-        NGP_CHECK_LAUNCH();
-    }
+    if (increment_step) return launch_step_inc(step_dev, st);
     return 0;
 }
 

@@ -460,9 +460,7 @@ class Trainer:
             return self.set_batch(rays_o, rays_d, rgb_gt)
         nxt = 1 - self._cur if (self._inflight or self._premarched) else self._cur
         st_ = self._sets[nxt]
-        ev = self._ev_set[nxt]
-        if ev is not None:
-            self._side.wait_event(ev)  # the set's last reader (the compute graph two steps back)
+        self._side.wait_event(self._ev_set[nxt])  # the set's last reader (the compute two steps back)
         with torch.cuda.stream(self._side):
             st_["rays_o"].copy_(rays_o, non_blocking=True)
             st_["rays_d"].copy_(rays_d, non_blocking=True)
@@ -634,9 +632,14 @@ class Trainer:
                               reads set i, accumulates into gradient buffer b
             g_update[b]     = [Adam], or for N > 1 the self-synchronising exchange kernel reducing buffer b and clearing
                               buffer 1-b (the NCCL modes launch their collectives eagerly)
+            g_step[i][b]    = g_compute[i][b] + g_update[b] as ONE graph, where no collective sits between them (one GPU,
+                              "p2p", "nvls"): the kernels of the chain are programmatic dependents of each other
+                              (common.cuh), and a graph boundary would drain the GPU between the scatter and the optimiser.
+                              An external event-record node after the scatter marks set i as read (_ev_set[i]).
+        train_step() replays g_step, or the split pair when an after_backward hook needs the boundary.
         The front of a step (batch assembly + march) depends on the rays, the jitter and the occupancy bitfield but
         NOT on the weights, so train_step() replays the NEXT step's g_prepare into the other buffer set on a side
-        stream while this step's g_compute and g_update run on the main stream (except across an occupancy refresh,
+        stream while this step's compute and optimiser run on the main stream (except across an occupancy refresh,
         whose new bitfield the next march must see -- the reference's ordering, train.py:160-163)."""
         dev = self.dev
         s = torch.cuda.Stream(dev)
@@ -674,15 +677,54 @@ class Trainer:
         elif self.ddp not in ("p2p_host", "zero"):
             self._gcur = 0
             self.g_update = [self._capture_graph(self.optimizer_step)]
+        # the moment set i's last reader (a step's compute) is done: the next march into set i waits for it
+        self._ev_set = [torch.cuda.Event(external=True) for _ in range(2)]
+        self.g_step = None
+        if self.ddp in ("none", "p2p", "nvls"):
+            fork = torch.cuda.Stream(dev)
+            self.g_step = []
+            for i in range(2):
+                self._cur = i
+                per_buf = []
+                for b in range(self._n_gbuf):
+                    self._gcur = b
+                    per_buf.append(self._capture_graph(lambda: self._compute_update(fork)))
+                self.g_step.append(per_buf)
         self._cur, self._gcur = keep
         self.graph = True
         self._graph_samples = sample
         self._side = torch.cuda.Stream(dev)
-        self._ev_compute = torch.cuda.Event()
-        self._ev_set = [None, None]
         self._staged = None
         self._inflight = False
         self._premarched = False
+
+    def _compute_update(self, fork):
+        """what g_step records: the compute, then the optimiser straight after the scatter on the main stream; the event
+        that set _cur is read hangs off the scatter on a forked branch (`fork`), so that no graph node sits between the
+        scatter and the optimiser's kernel"""
+        main = torch.cuda.current_stream(self.dev)
+        self._compute()
+        fork.wait_stream(main)
+        self._ev_set[self._cur].record(fork)
+        if self.ddp in ("p2p", "nvls"):
+            self._launch_fused()
+        else:
+            self.optimizer_step()
+        main.wait_stream(fork)
+
+    def _graph_compute_update(self, after_backward):
+        """the compute and the optimiser of a captured step on the main stream; _ev_set[_cur] is recorded once the compute
+        is done"""
+        if after_backward is None and self.g_step is not None:
+            self._replay(self.g_step[self._cur][self._gcur])
+            if self._n_gbuf == 2:
+                self._gcur ^= 1
+            return
+        self._replay(self.g_compute[self._cur][self._gcur])
+        if after_backward is not None:
+            after_backward(self)
+        self._ev_set[self._cur].record(torch.cuda.current_stream(self.dev))
+        self._graph_update()
 
     def _graph_update(self):
         """the optimiser half of a captured step on the main stream"""
@@ -723,13 +765,7 @@ class Trainer:
             main.wait_stream(self._side)
             if refresh:  # staged ahead of a refresh: march now, against the refreshed grid (the reference's ordering)
                 self._replay(self.g_prepare[self._cur])
-            self._replay(self.g_compute[self._cur][self._gcur])
-            if after_backward is not None:
-                after_backward(self)
-            if self._ev_set[self._cur] is None:
-                self._ev_set[self._cur] = torch.cuda.Event()
-            self._ev_set[self._cur].record(main)
-            self._graph_update()
+            self._graph_compute_update(after_backward)
             self._premarched = False
             self._inflight = True
             self.host_step += 1
@@ -741,19 +777,15 @@ class Trainer:
         # deep pipeline: the next step's batch + march into the OTHER set (side stream) under this whole step
         ahead = sample and ((self.host_step + 1) % self.update_interval != 0)
         if ahead:
-            # the other set's last reader is the previous step's g_compute: once that is done (and this step's march, if it
+            # the other set's last reader is the previous step's compute: once that is done (and this step's march, if it
             # ran on the main stream, is enqueued) the next march may start -- it does not wait for the optimiser
             if self._premarched:
-                self._side.wait_event(self._ev_compute)
+                self._side.wait_event(self._ev_set[1 - self._cur])
             else:
                 self._side.wait_stream(main)
             with torch.cuda.stream(self._side):
                 self._replay(self.g_prepare[1 - self._cur])
-        self._replay(self.g_compute[self._cur][self._gcur])
-        if after_backward is not None:
-            after_backward(self)
-        self._ev_compute.record(main)
-        self._graph_update()
+        self._graph_compute_update(after_backward)
         if ahead:
             main.wait_stream(self._side)
         self._premarched = ahead

@@ -3,7 +3,9 @@
 ngp_trace_set() makes the step's entry points enqueue a one-thread kernel after each of their kernels that appends
 {id, %globaltimer}; the stamps are captured into the CUDA graphs, so the timeline is the graph-replayed, two-stream
 steady state. Each stamp adds to the launch chain, so the traced step is slower than the untraced one (both are
-printed); read it for WHERE time goes, not for absolute numbers.
+printed); read it for WHERE time goes, not for absolute numbers. The step's kernels are chained by programmatic dependent
+launch (a kernel starts under its predecessor's tail, csrc/common.cuh); a stamp kernel between two of them breaks that
+edge, so what the chain saves shows in the untraced step time only.
 
     python tools/step_timeline.py [steps] [n_steps_to_print] [ddp mode]
     python -m torch.distributed.run --nproc-per-node N ... tools/step_timeline.py 1200 3 nvls     (rank 0 prints)
