@@ -386,9 +386,11 @@ int ngp_update_density_grid(const NgpNet* net, float* density_grid /* (cascades,
 /* The same refresh in two halves, ngp_update_density_grid == pick then eval on one stream. `pick` needs only the OLD grid
  * and the seed (which cells, sorted in Morton order, and the jittered point in each; clears the scratch grid), so a trainer
  * runs it on a side stream any time after the previous refresh and only `eval` (density at the points, merge, threshold,
- * bitfield) sits between two training steps. A cell picked more than once is evaluated once, at its first pick's point
- * (the reference's index_put keeps an arbitrary one of the duplicates). Both halves must see the same workspace, cascades, grid_size, threshold and
- * warmup, and nothing else may touch the workspace in between. */
+ * bitfield) sits between two training steps. A cell picked more than once is evaluated once (the reference's index_put
+ * keeps an arbitrary one of the duplicates), at a point hashed from the cell's rank among the cascade's distinct picks in
+ * Morton order -- not from any of its pick slots. grid_size must be a power of two in [2, 1024], cascades in [1, 62] and
+ * cascades * grid_size^3 < 2^31; both halves return NGP_EINVAL otherwise. Both halves must see the same workspace,
+ * cascades, grid_size, threshold and warmup, and nothing else may touch the workspace in between. */
 int ngp_update_density_grid_pick(const float* density_grid, int cascades, int grid_size, float scale, float density_threshold,
                                  int warmup, uint32_t seed, void* workspace, size_t workspace_bytes, void* stream);
 int ngp_update_density_grid_eval(const NgpNet* net, float* density_grid, uint8_t* density_bitfield, const float* count_grid,

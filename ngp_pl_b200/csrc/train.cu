@@ -1111,7 +1111,8 @@ __global__ void k_grid_pick_cells(const GridUpd u, int c, const int* __restrict_
 // One jittered point inside each picked cell. Warm-up (keys == nullptr): slot i of cascade c is cell i. Otherwise `keys`
 // are this cascade's picked cells sorted AND de-duplicated (*n_keys of them): a cell picked more than once is evaluated once
 // -- the reference's index_put keeps an arbitrary one of the duplicates' values, and with ~150 k occupied cells drawn
-// 524 k times most picks ARE duplicates -- so the density pass runs over the distinct cells only. Slots of successive
+// 524 k times most picks ARE duplicates -- so the density pass runs over the distinct cells only; the point is hashed from
+// i, the cell's rank among the distinct sorted picks, not from any pick slot. Slots of successive
 // cascades are appended: tot[c] = first slot of cascade c, tot[cascades] = number of slots of this refresh.
 // cell_idx = c * g3 + cell (-1: nothing to evaluate).
 __global__ void k_grid_jitter(const GridUpd u, int c, const uint32_t* __restrict__ keys, const int* __restrict__ n_keys,
@@ -1262,6 +1263,13 @@ extern "C" size_t ngp_update_grid_workspace(int cascades, int grid_size) {
     if (cascades < 1 || grid_size < 1) return 0;
     return grid_ws(nullptr, cascades, (size_t)grid_size * grid_size * grid_size).total;
 }
+// Arguments both halves accept: Morton indices tile [0, G^3) only when G is a power of two (otherwise the warm-up decodes
+// slots to coordinates >= G and the marcher's morton_encode3 indexes past the cascade); at most 62 cascades, because
+// tot[63] holds the distinct-key count; cell_idx = c * g3 + cell must fit an int.
+static bool grid_args_ok(int cascades, int grid_size) {
+    if (cascades < 1 || cascades > 62 || grid_size < 2 || grid_size > 1024 || (grid_size & (grid_size - 1)) != 0) return false;
+    return (int64_t)cascades * grid_size * grid_size * grid_size <= 0x7fffffffll;
+}
 
 // First half of the refresh: everything that depends on the OLD density grid and the seed but not on the weights -- which
 // cells to re-evaluate (sorted) and a jittered point in each, plus clearing the scratch grid. A trainer runs it on a side
@@ -1269,8 +1277,7 @@ extern "C" size_t ngp_update_grid_workspace(int cascades, int grid_size) {
 extern "C" int ngp_update_density_grid_pick(const float* density_grid, int cascades, int grid_size, float scale,
                                             float density_threshold, int warmup, uint32_t seed, void* workspace,
                                             size_t workspace_bytes, void* stream) {
-    if (!density_grid || !workspace || cascades < 1 || cascades > 62 || grid_size < 2 || grid_size > 1024) return NGP_EINVAL;
-    if ((int64_t)cascades * grid_size * grid_size * grid_size > 0x7fffffffll) return NGP_EINVAL;  // cell_idx = c * g3 + cell
+    if (!density_grid || !workspace || !grid_args_ok(cascades, grid_size)) return NGP_EINVAL;
     if (workspace_bytes < ngp_update_grid_workspace(cascades, grid_size)) return NGP_EINVAL;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t g3 = (size_t)grid_size * grid_size * grid_size;
@@ -1315,8 +1322,7 @@ extern "C" int ngp_update_density_grid_pick(const float* density_grid, int casca
 extern "C" int ngp_update_density_grid_eval(const NgpNet* net, float* density_grid, uint8_t* density_bitfield,
                                             const float* count_grid, int cascades, int grid_size, float density_threshold,
                                             int warmup, float decay, void* workspace, size_t workspace_bytes, void* stream) {
-    if (!net || !density_grid || !density_bitfield || !workspace || cascades < 1 || grid_size < 2 || grid_size > 1024)
-        return NGP_EINVAL;
+    if (!net || !density_grid || !density_bitfield || !workspace || !grid_args_ok(cascades, grid_size)) return NGP_EINVAL;
     if (workspace_bytes < ngp_update_grid_workspace(cascades, grid_size)) return NGP_EINVAL;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t g3 = (size_t)grid_size * grid_size * grid_size;

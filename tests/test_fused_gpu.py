@@ -199,13 +199,8 @@ def test_update_density_grid_semantics():
     assert (grid[0] > 0).all()
     assert ratio.median().item() == pytest.approx(1.0, abs=0.05)
     assert ((ratio > 0.5) & (ratio < 2.0)).float().mean().item() > 0.99
-    mean = grid[grid > 0].mean().item()
-    want = torch.zeros_like(model.density_bitfield)
-    vren.packbits(grid, min(mean, thr), want)
-    diff = (want ^ model.density_bitfield).to(torch.int32)
-    flipped = sum(((diff >> b) & 1).sum().item() for b in range(8))
-    assert flipped <= 1e-3 * G3, "bitfield disagrees with packbits(grid, min(mean, thr)) on %d cells" % flipped
-    # regular refresh: cells marked -1 stay -1, nothing decays faster than `decay`, sampled cells rise to sigma
+    # the bitfield, the picks, the merge and the mean are pinned cell by cell in test_grid_refresh_gpu.py
+    # regular refresh: cells marked -1 stay -1, nothing decays faster than `decay`
     model.density_grid[0, :1000] = -1
     before = model.density_grid.clone()
     tr.host_step = 17
@@ -213,10 +208,7 @@ def test_update_density_grid_semantics():
     torch.cuda.synchronize()
     after = model.density_grid
     assert (after[0, :1000] == -1).all()
-    rest = before[0, 1000:]
-    assert (after[0, 1000:] >= 0.95 * rest - 1e-6).all()
-    grown = (after[0, 1000:] > rest * 0.95 + 1e-6).float().mean().item()
-    assert 0.2 < grown < 0.55  # ~M uniform + ~M occupied of G^3 cells, with collisions
+    assert (after[0, 1000:] >= 0.95 * before[0, 1000:] - 1e-6).all()
     # different seeds/steps pick different cells
     tr.host_step = 33
     b2 = model.density_grid.clone()
