@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 7
+#define NGP_ABI_VERSION 8
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -342,6 +342,22 @@ int ngp_adam_step_fused(int world, int rank, const uint64_t* peer_grads, const u
                         float* exp_avg, float* exp_avg_sq, int64_t n, float* zero_buf, uint32_t* sync,
                         const float* lr_dev, int32_t* step_dev, float beta1, float beta2, float eps,
                         int increment_step, void* stream);
+
+/* Per-step training log (Trainer(log_rows=R); the reference logs train/loss, train/psnr, train/rm_s, train/vr_s and lr
+ * every step, train.py:175-183): one single-block kernel that writes one row of a caller-owned device ring
+ * log[rows][8] (int32 words) without any host counter, so that one captured CUDA graph writes the right row on every
+ * replay. Launch it after the step's optimiser, which has advanced *step_dev: the row is (*step_dev - 1) mod rows and
+ * holds
+ *   [0] scalars[2] (sum of squared errors, fp32 bits)   [1] scalars[3] (sum of opacity entropy, fp32 bits)
+ *   [2] counters[2] (ray-marched samples)                [3] counters[3] (volume-rendered samples)
+ *   [4] counters[5] (samples the backward visited)       [5] *lr_dev (fp32 bits)
+ *   [6] sum of dist_loss[0 .. n_dist) (fp32 bits; 0 when n_dist == 0, fixed-order double reduction)
+ *   [7] *step_dev - 1 (the step's index)
+ * scalars / counters: the step's NgpTrainBuffers fields. dist_loss may be NULL when n_dist == 0. Launched as a
+ * programmatic dependent of the kernel before it; it reads nothing before that kernel has completed, and the kernel
+ * after it starts once it has completed. */
+int ngp_train_log_step(const float* scalars, const int32_t* counters, const float* lr_dev, const int32_t* step_dev,
+                       const float* dist_loss, int64_t n_dist, int32_t* log, int rows, void* stream);
 
 /* Batch assembly on the device (reference train.py:78-91 + datasets/ray_utils.py:46-70 + base.py:22-30):
  * rays_d = directions[pix] @ R^T, rays_o = c2w[:,3], rgb_gt = images[img, pix] / 255. */

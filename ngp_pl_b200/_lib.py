@@ -9,7 +9,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 7  #NGP_ABI_VERSION in include/ngp_b200.h
+ABI_VERSION = 8  #NGP_ABI_VERSION in include/ngp_b200.h
 
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
@@ -160,6 +160,7 @@ SIGNATURES = {
     "ngp_adam_step": (_i, [_P, _P, _P, _P, _P, _i64, _P, _P, _f, _f, _f, _f, _i, _P]),
     "ngp_adam_step_p2p": (_i, [_i, _i, _P, _P, _P, _P, _P, _i64, _P, _P, _f, _f, _f, _i, _P]),
     "ngp_adam_step_fused": (_i, [_i, _i, _P, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P, _i64, _P, _P, _P, _P, _f, _f, _f, _i, _P]),
+    "ngp_train_log_step": (_i, [_P, _P, _P, _P, _P, _i64, _P, _i, _P]),
     "ngp_gen_rays": (_i, [_P, _P, _P, _P, _P, _i64, _i, _P, _P, _P, _P]),
     "ngp_sample_rays": (_i, [_P, _P, _P, _i, _i64, _i, C.c_uint32, C.c_uint32, _P, _P, _P, _P, _P, _P]),
     "ngp_sample_rays_ex": (_i, [_P, _P, _P, _i, _i, _i, _i64, _i, C.c_uint32, C.c_uint32, _P, _P, _P, _P, _P, _P]),

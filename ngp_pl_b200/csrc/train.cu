@@ -556,6 +556,46 @@ static int launch_step_inc(int* step_dev, cudaStream_t st) {
     return 0;
 }
 
+// One row of the per-step training log (ngp_train_log_step). The last link of the step's chain: it waits for the
+// optimiser (which advanced the step counter) and does not trigger its successor early, so the next step's kernels
+// start only once the row is written and the quantities it read are no longer needed.
+constexpr int kLogThreads = 256;
+__global__ void __launch_bounds__(kLogThreads) k_train_log(const float* __restrict__ scalars, const int* __restrict__ counters,
+                                                           const float* __restrict__ lr_dev, const int* __restrict__ step_dev,
+                                                           const float* __restrict__ dist_loss, int64_t n_dist,
+                                                           int* __restrict__ log, int rows) {
+    pdl_wait();
+    __shared__ double part[kLogThreads / NGP_WARP];
+    double s = 0.0;
+    for (int64_t i = threadIdx.x; i < n_dist; i += kLogThreads) s += (double)dist_loss[i];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & (NGP_WARP - 1)) == 0) part[threadIdx.x / NGP_WARP] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int w = 0; w < kLogThreads / NGP_WARP; ++w) t += part[w];
+        const int step = *step_dev - 1;
+        int r = step % rows;
+        if (r < 0) r += rows;
+        int4* row = reinterpret_cast<int4*>(log + 8 * (int64_t)r);
+        row[0] = make_int4(__float_as_int(scalars[2]), __float_as_int(scalars[3]), counters[2], counters[3]);
+        row[1] = make_int4(counters[5], __float_as_int(*lr_dev), __float_as_int((float)t), step);
+    }
+}
+
+extern "C" int ngp_train_log_step(const float* scalars, const int32_t* counters, const float* lr_dev, const int32_t* step_dev,
+                                  const float* dist_loss, int64_t n_dist, int32_t* log, int rows, void* stream) {
+    if (!scalars || !counters || !lr_dev || !step_dev || !log || rows < 1 || n_dist < 0 || (n_dist > 0 && !dist_loss))
+        return NGP_EINVAL;
+    if (((uintptr_t)log) & 15) return NGP_EINVAL;
+    cudaStream_t st = (cudaStream_t)stream;
+    NGP_CUDA(ngp_launch_pdl(k_train_log, 1, kLogThreads, 0, st, scalars, counters, lr_dev, step_dev, dist_loss, n_dist, log,
+                            rows));
+    NGP_CHECK_LAUNCH();
+    return 0;
+}
+
 extern "C" int ngp_adam_step(float* params, float* grads, float* exp_avg, float* exp_avg_sq, uint16_t* params_half, int64_t n,
                              const float* lr_dev, int32_t* step_dev, float beta1, float beta2, float eps, float grad_mul,
                              int increment_step, void* stream) {

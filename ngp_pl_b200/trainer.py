@@ -96,6 +96,51 @@ class CosineAnnealingLR:
         return self.lr_at_epoch(step // self.steps_per_epoch)
 
 
+def log_ring_spans(first, n, rows):
+    """The per-step log keeps step k in row k % rows of its ring. Returns the ring slices [lo, hi) that hold steps
+    first .. first + n - 1, in step order (two slices when the range wraps). n may not exceed rows: older steps of the
+    range would already be overwritten."""
+    if n < 0 or rows < 1:
+        raise ValueError("log_ring_spans: n must be >= 0 and rows >= 1, got n=%d rows=%d" % (n, rows))
+    if n > rows:
+        raise RuntimeError("log_ring_spans: %d steps do not fit a ring of %d rows" % (n, rows))
+    spans, s = [], first
+    while n > 0:
+        lo = s % rows
+        k = min(n, rows - lo)
+        spans.append((lo, lo + k))
+        s += k
+        n -= k
+    return spans
+
+
+def log_rows_to_stats(rows, n_rays, lambda_opacity, lambda_distortion=0.0, live=True):
+    """Decode rows of the per-step log ((n, 8) int32 numpy, the layout of ngp_train_log_step) into the dicts
+    Trainer.stats() returns after that step -- the same formulas on the same fp32 values, so loss, mse, psnr and the
+    sample counts are bitwise stats()'s -- plus 'step' (0-based index) and 'lr' (the fp32 rate the step's Adam used).
+    lambda_opacity must be the value the kernels saw (Trainer.cfg.lambda_opacity); live: whether the trainer skips dead
+    samples (bw_samples is rm_samples otherwise). With lambda_distortion > 0, 'distortion' is the mean of the step's
+    distortion loss times lambda_distortion from a double sum (stats() takes torch's fp32 mean), and is part of 'loss'."""
+    import numpy as np
+    rows = np.ascontiguousarray(rows, dtype=np.int32).reshape(-1, 8)
+    f = rows.view(np.float32)
+    out = []
+    for r, x in zip(rows.tolist(), f.tolist()):
+        n = n_rays
+        mse = x[0] / (3 * n)
+        loss = mse + lambda_opacity * x[1] / n
+        d = dict(rm_samples=r[2], vr_samples=r[3], bw_samples=r[4] if live else r[2], mse=mse,
+                 psnr=-10 * math.log10(max(mse, 1e-12)))
+        if lambda_distortion > 0:
+            d["distortion"] = lambda_distortion * (x[6] / n)
+            loss += d["distortion"]
+        d["loss"] = loss
+        d["step"] = r[7]
+        d["lr"] = x[5]
+        out.append(d)
+    return out
+
+
 _SET_FIELDS = ("rays_o", "rays_d", "rgb_gt", "noise", "n_samples", "offsets", "counters", "ray_idx", "ts", "deltas", "bg")
 
 
@@ -104,7 +149,9 @@ class Trainer:
                  T_threshold=1e-4, betas=(0.9, 0.999), eps=1e-15, max_total_samples=None, update_interval=16,
                  warmup_steps=256, process_group=None, world_size=1, rank=0, seed=0, materialize_ws=False, ddp="nccl",
                  lambda_distortion=0.0, skip_dead_samples=True, fused_loss=True, random_bg=False, erode=False,
-                 lr_schedule=None, pick_ahead=True, ray_sampling_strategy="all_images"):
+                 lr_schedule=None, pick_ahead=True, ray_sampling_strategy="all_images", log_rows=0):
+        if int(log_rows) < 0:
+            raise ValueError("Trainer: log_rows must be >= 0 (0 = no per-step log), got %r" % (log_rows,))
         if ray_sampling_strategy not in ("all_images", "same_image"):
             raise ValueError("Trainer: ray_sampling_strategy must be 'all_images' or 'same_image', got %r" % (ray_sampling_strategy,))
         self.ray_sampling_strategy = ray_sampling_strategy  # reference opt.py:34-39
@@ -209,6 +256,13 @@ class Trainer:
             model.rgb_net._half = _FixedHalf(self.Ph[self.n_enc:])
             self.lr_dev = torch.full((1,), self.lr, device=dev, dtype=torch.float32)
             self.step_dev = torch.zeros(1, device=dev, dtype=torch.int32)
+            # per-step log (drain_log): ring of log_rows rows written on the device by ngp_train_log_step
+            self.log_rows = int(log_rows)
+            self.log_ring = torch.zeros(self.log_rows, 8, device=dev, dtype=torch.int32) if self.log_rows else None
+            self._log_next = 0        # first step not yet enqueued for a copy
+            self._log_pending = []    # (first step, n, pinned rows, copy-done event), oldest first
+            self._log_stream = None
+            self._log_quiet = False
 
             # ---- network descriptor pointing at the flat fp16 copy -----------------------------------------
             net = _lib.NgpNet()
@@ -601,6 +655,19 @@ class Trainer:
     def _update(self):
         self.allreduce()
         self.optimizer_step()
+        self._log_step()
+
+    def _log_step(self):
+        """with log_rows > 0: the step's row of the log ring, after the optimiser (which advanced step_dev) on the current
+        stream; nothing at all otherwise"""
+        if self.log_ring is None or self._log_quiet:
+            return
+        dist = self.dist_loss if self.lambda_distortion > 0 else None
+        rc = _lib.lib().ngp_train_log_step(self.scalars.data_ptr(), self.counters.data_ptr(), self.lr_dev.data_ptr(),
+                                           self.step_dev.data_ptr(), None if dist is None else dist.data_ptr(),
+                                           0 if dist is None else dist.numel(), self.log_ring.data_ptr(), self.log_rows,
+                                           self._st())
+        _lib.check(rc, "train_log_step")
 
     def _step_body(self, sample):
         self._prepare(sample)
@@ -649,7 +716,11 @@ class Trainer:
             # one eager run so lazy initialisation (cudaFuncSetAttribute, NCCL / symmetric-memory setup) is done
             saved = [t.clone() for t in state]
             gcur = self._gcur
-            self._step_body(sample)
+            self._log_quiet = True  # a step that is undone below writes no log row
+            try:
+                self._step_body(sample)
+            finally:
+                self._log_quiet = False
             if self.ddp == "p2p_host":
                 self.hG.barrier(channel=0)
             for t, v in zip(state, saved):
@@ -710,6 +781,7 @@ class Trainer:
             self._launch_fused()
         else:
             self.optimizer_step()
+        self._log_step()
         main.wait_stream(fork)
 
     def _graph_compute_update(self, after_backward):
@@ -727,19 +799,23 @@ class Trainer:
         self._graph_update()
 
     def _graph_update(self):
-        """the optimiser half of a captured step on the main stream"""
+        """the optimiser half of a captured step on the main stream (+ the log row, launched here because g_update is
+        shared by both buffer sets while the row reads the step's own set)"""
         self.allreduce()
         if self.g_update is None:
             self.optimizer_step()
-            return
-        self._replay(self.g_update[self._gcur])
-        if self._n_gbuf == 2:
-            self._gcur ^= 1
+        else:
+            self._replay(self.g_update[self._gcur])
+            if self._n_gbuf == 2:
+                self._gcur ^= 1
+        self._log_step()
 
     def train_step(self, sample=True, after_backward=None):
         """one full training step incl. the occupancy refresh cadence of reference train.py:160-163. after_backward(self),
         if given, is called once the step's gradients (self.G) are complete and before the optimiser consumes and
         clears them"""
+        if self._log_pending:
+            self._log_guard()
         if self.lr_schedule is not None:
             lr = self.lr_schedule.lr_at_step(self.host_step)
             if lr != self.lr:
@@ -804,3 +880,61 @@ class Trainer:
             loss += out["distortion"]
         out["loss"] = loss
         return out
+
+    # ---- the per-step log (Trainer(log_rows=R)) -------------------------------------------------------------
+    def drain_log(self, wait=False):
+        """Every step's stats() without synchronising the host. Enqueues one device-to-host copy of the log rows written
+        since the last drain (on a side stream, behind an event recorded on the current stream, into pinned memory) and
+        returns, in step order, the rows of earlier drains whose copies have completed, as the dicts of
+        log_rows_to_stats(): stats()'s keys plus 'step' and 'lr'. wait=True also waits for the copies still in flight
+        (for tests and the end of a run). Call it at least every log_rows steps: if more steps have passed, their oldest
+        rows are overwritten and it raises (the rows of the earlier drains are kept for the next call)."""
+        if self.log_ring is None:
+            raise RuntimeError("Trainer.drain_log: the per-step log is off (construct the Trainer with log_rows > 0)")
+        R = self.log_rows
+        first, n = self._log_next, self.host_step - self._log_next
+        if n > R:
+            self._log_next = self.host_step
+            raise RuntimeError("Trainer.drain_log: %d steps since the last drain, the log ring holds %d: the rows of steps "
+                               "%d..%d are overwritten (drain at least every log_rows steps)" % (n, R, first, self.host_step - R - 1))
+        if n > 0:
+            with torch.cuda.device(self.dev):
+                main = torch.cuda.current_stream(self.dev)
+                if self._log_stream is None:
+                    self._log_stream = torch.cuda.Stream(self.dev)
+                    self.log_ring.record_stream(self._log_stream)
+                ready = torch.cuda.Event()
+                ready.record(main)
+                self._log_stream.wait_event(ready)
+                host = torch.empty(n, 8, dtype=torch.int32, pin_memory=True)
+                at = 0
+                with torch.cuda.stream(self._log_stream):
+                    for lo, hi in log_ring_spans(first, n, R):
+                        host[at:at + hi - lo].copy_(self.log_ring[lo:hi], non_blocking=True)
+                        at += hi - lo
+                done = torch.cuda.Event()
+                done.record(self._log_stream)
+            self._log_pending.append((first, n, host, done))
+            self._log_next = self.host_step
+        out = []
+        while self._log_pending:
+            first, n, host, done = self._log_pending[0]
+            if wait:
+                done.synchronize()
+            elif not done.query():
+                break
+            self._log_pending.pop(0)
+            rows = log_rows_to_stats(host.numpy(), self.n_rays, self.cfg.lambda_opacity, self.lambda_distortion,
+                                     self.live_idx is not None)
+            if [r["step"] for r in rows] != list(range(first, first + n)):
+                raise RuntimeError("Trainer.drain_log: the log rows are not those of steps %d..%d (was the optimiser "
+                                   "stepped outside train_step?)" % (first, first + n - 1))
+            out += rows
+        return out
+
+    def _log_guard(self):
+        """a copy still in flight may hold the row the coming step overwrites: the step waits for that copy"""
+        s = self.host_step - self.log_rows
+        for first, n, _, done in self._log_pending:
+            if first <= s < first + n:
+                torch.cuda.current_stream(self.dev).wait_event(done)
