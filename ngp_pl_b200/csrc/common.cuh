@@ -79,6 +79,21 @@ static inline cudaError_t ngp_launch_pdl(void (*kernel)(KArgs...), dim3 grid, di
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
+// Let Kernel use `bytes` (> 48 KB) of dynamic shared memory on the current device. The opt-in is a per-device function
+// attribute and one process may drive several GPUs, so it is set once per device (device ordinals past 63: every call).
+template <auto Kernel>
+static inline cudaError_t ngp_smem_opt_in(int bytes) {
+    static unsigned char set[64] = {0};
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    const bool cached = dev >= 0 && dev < 64;
+    if (cached && __atomic_load_n(&set[dev], __ATOMIC_ACQUIRE)) return cudaSuccess;
+    e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess && cached) __atomic_store_n(&set[dev], 1, __ATOMIC_RELEASE);
+    return e;
+}
+
 // Number of SMs of the current device (132 on H100 SXM); cached per process.
 static inline int ngp_sm_count() {
     static int sms = 0;

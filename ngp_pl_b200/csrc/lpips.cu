@@ -261,12 +261,7 @@ template <int BM, int BN, int BK, int WM, int WN>
 static int lp_conv_launch(const __half* in, const __half* wt, const float* bias, __half* out, int H, int W, int Cin,
                           int Cout, cudaStream_t st) {
     using T = LpConv<BM, BN, BK, WM, WN>;
-    static bool attr = false;
-    if (!attr) {
-        NGP_CUDA(cudaFuncSetAttribute(k_lpips_conv<BM, BN, BK, WM, WN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)T::SMEM));
-        attr = true;
-    }
+    NGP_CUDA((ngp_smem_opt_in<k_lpips_conv<BM, BN, BK, WM, WN>>((int)T::SMEM)));
     const dim3 grid(ngp_div_up(2 * (int64_t)H * W, BM), Cout / BN);
     k_lpips_conv<BM, BN, BK, WM, WN><<<grid, LP_THREADS, T::SMEM, st>>>(in, wt, bias, out, H, W, Cin, Cout);
     NGP_CHECK_LAUNCH();

@@ -235,12 +235,7 @@ extern "C" size_t ngp_image_metrics_workspace(int H, int W) {
 template <bool GT_U8, bool SSIM>
 static int met_launch(dim3 grid, cudaStream_t st, const float* pred, const void* gt, int H, int W, const MetWindow& win,
                       double c1, double c2, double* out_sse, double* out_ssim, void* workspace) {
-    static bool attr = false;
-    if (!attr) {
-        NGP_CUDA(cudaFuncSetAttribute(k_image_metrics<GT_U8, SSIM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)sizeof(MetSmem)));
-        attr = true;
-    }
+    NGP_CUDA((ngp_smem_opt_in<k_image_metrics<GT_U8, SSIM>>((int)sizeof(MetSmem))));
     k_image_metrics<GT_U8, SSIM><<<grid, MET_THREADS, sizeof(MetSmem), st>>>(
         pred, gt, H, W, win, c1, c2, out_sse, out_ssim, reinterpret_cast<unsigned int*>(workspace),
         reinterpret_cast<double2*>(reinterpret_cast<unsigned char*>(workspace) + MET_HEADER));

@@ -7,11 +7,10 @@
 //   ngp_enc_backward     tcnn.NetworkWithInputEncoding backward from dL/dh (N,16): weight gradients +
 //                        feature gradients for ngp_net_backward_scatter (its forward is ngp_net_forward
 //                        with want_rgb = 0 and h_out)
-// The fused NGP kernels (network.cu) are the hot path; these reuse the same warp-level building blocks
-// (mlp.cuh) in the simple 8-warp / stage-everything form.
+// The fused NGP kernels (network.cu) are the hot path; these run the same network chains (network.cuh) in the simple
+// 8-warp / stage-everything form, with their own mma.sync weight-gradient loops.
 #include "common.cuh"
-#include "hashgrid.cuh"
-#include "mlp.cuh"
+#include "network.cuh"
 #include "../../include/ngp_b200.h"
 
 // ---------------------------------------------------------------------------------------------------
@@ -40,8 +39,6 @@ extern "C" int ngp_sh_encode(const float* u01, int64_t n, uint16_t* out_half, vo
 #define MOD_WARPS 8
 #define MOD_THREADS (MOD_WARPS * 32)
 #define MOD_ROWS (MOD_WARPS * 16)
-
-__device__ __forceinline__ float lo_h(uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u & 0xffffu))); }
 
 // A fragments (K = 32) of 16 rows of a row-major fp16 matrix X (n, 32) in global memory
 __device__ __forceinline__ void load_rows32(const __half* __restrict__ X, int64_t base, int64_t n, uint32_t (&A)[1][2][4], int g, int q) {
@@ -112,33 +109,18 @@ k_mlp_rgb_fwd(const __half* __restrict__ wr, const __half* __restrict__ X, int64
         const int64_t base = tile * 16;
         uint32_t inA[1][2][4];
         load_rows32(X, base, n, inA, g, q);
-        uint32_t r1A[1][4][4], r2A[1][4][4];
-        {
-            float c[1][8][4];
-            mlp_layer<1, 32, 64, LD32>(inA, sw.w1r, c, g, q);
-            relu_to_frag<1, 64>(c, r1A);
-        }
-        {
-            float c[1][8][4];
-            mlp_layer<1, 64, 64, LD64>(r1A, sw.w2r, c, g, q);
-            relu_to_frag<1, 64>(c, r2A);
-        }
         float oC[1][1][4];
-        mlp_layer<1, 64, 8, LD64>(r2A, sw.w3r, oC, g, q);
+        color_mlp<1>(inA, sw.w1r, sw.w2r, sw.w3r, oC, g, q, [](int, const auto&) {});
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int64_t row = base + g + 8 * h;
             if (row >= n || q > 1) continue;
-            float a = oC[0][0][2 * h], b = oC[0][0][2 * h + 1];
-            if (act == 1) {
-                a = 1.0f / (1.0f + __expf(-a));
-                b = 1.0f / (1.0f + __expf(-b));
-            }
+            const __half2 o = rgb_out(oC[0][0][2 * h], oC[0][0][2 * h + 1], act);
             if (q == 0) {
-                out3[3 * row] = __float2half_rn(a);
-                out3[3 * row + 1] = __float2half_rn(b);
+                out3[3 * row] = __low2half(o);
+                out3[3 * row + 1] = __high2half(o);
             } else {
-                out3[3 * row + 2] = __float2half_rn(a);
+                out3[3 * row + 2] = __low2half(o);
             }
         }
     }
@@ -198,18 +180,13 @@ k_mlp_rgb_bwd(const __half* __restrict__ wr, const __half* __restrict__ X, const
         uint32_t inA[1][2][4];
         load_rows32(X, base, n, inA, g, q);
         uint32_t r1A[1][4][4], r2A[1][4][4];
-        {
-            float c[1][8][4];
-            mlp_layer<1, 32, 64, LD32>(inA, S.w.w1r, c, g, q);
-            relu_to_frag<1, 64>(c, r1A);
-        }
-        {
-            float c[1][8][4];
-            mlp_layer<1, 64, 64, LD64>(r1A, S.w.w2r, c, g, q);
-            relu_to_frag<1, 64>(c, r2A);
-        }
         float oC[1][1][4];
-        mlp_layer<1, 64, 8, LD64>(r2A, S.w.w3r, oC, g, q);
+        color_mlp<1>(inA, S.w.w1r, S.w.w2r, S.w.w3r, oC, g, q, [&](int l, const uint32_t (&r)[1][4][4]) {
+#pragma unroll
+            for (int kt = 0; kt < 4; ++kt)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) (l == 1 ? r1A : r2A)[0][kt][e] = r[0][kt][e];
+        });
         uint32_t doutA[1][1][4];
         doutA[0][0][2] = 0u; doutA[0][0][3] = 0u;
 #pragma unroll
@@ -217,13 +194,8 @@ k_mlp_rgb_bwd(const __half* __restrict__ wr, const __half* __restrict__ X, const
             const int64_t row = base + g + 8 * h;
             float d0 = 0.f, d1 = 0.f;
             if (row < n && q < 2) {
-                float s0 = 1.f, s1 = 1.f;
-                if (act == 1) {
-                    const float o0 = __half2float(__float2half_rn(1.0f / (1.0f + __expf(-oC[0][0][2 * h]))));
-                    const float o1 = __half2float(__float2half_rn(1.0f / (1.0f + __expf(-oC[0][0][2 * h + 1]))));
-                    s0 = o0 * (1.0f - o0);
-                    s1 = o1 * (1.0f - o1);
-                }
+                float s0 = oC[0][0][2 * h], s1 = oC[0][0][2 * h + 1];
+                rgb_out_grad(s0, s1, act);
                 if (q == 0) {
                     d0 = __ldg(dL_dout3 + 3 * row) * s0 * scale;
                     d1 = __ldg(dL_dout3 + 3 * row + 1) * s1 * scale;
@@ -289,11 +261,7 @@ extern "C" int ngp_mlp_rgb_backward(const uint16_t* rgb_params_h, const uint16_t
                                     int rgb_act, const float* loss_scale, float* dL_dx, float* grad_rgb, void* stream) {
     if (n < 0 || !rgb_params_h || !grad_rgb || (n > 0 && (!x_half || !dL_dout3)) || (((uintptr_t)dL_dx) & 7)) return NGP_EINVAL;
     if (n == 0) return 0;
-    static bool attr = false;
-    if (!attr) {
-        NGP_CUDA(cudaFuncSetAttribute(k_mlp_rgb_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RgbBwdSmem)));
-        attr = true;
-    }
+    NGP_CUDA(ngp_smem_opt_in<k_mlp_rgb_bwd>((int)sizeof(RgbBwdSmem)));
     const int64_t n_blks = ((n + 15) / 16 + MOD_WARPS - 1) / MOD_WARPS;
     const int grid = (int)(n_blks < (int64_t)ngp_sm_count() ? n_blks : ngp_sm_count());
     k_mlp_rgb_bwd<<<grid, MOD_THREADS, sizeof(RgbBwdSmem), (cudaStream_t)stream>>>(
@@ -345,11 +313,7 @@ k_enc_bwd(const __half* __restrict__ wd, const uint4* __restrict__ feat_save, co
             featA[0][kt][0] = v.x; featA[0][kt][1] = v.y; featA[0][kt][2] = v.z; featA[0][kt][3] = v.w;
         }
         uint32_t hidA[1][4][4];
-        {
-            float c[1][8][4];
-            mlp_layer<1, 32, 64, LD32>(featA, S.w1d, c, g, q);
-            relu_to_frag<1, 64>(c, hidA);
-        }
+        density_hidden<1>(featA, S.w1d, hidA, g, q);
         uint32_t dhA[1][1][4];
         {
             float c[1][2][4];
@@ -413,11 +377,7 @@ extern "C" int ngp_enc_backward(const NgpNet* net, const NgpSamples* smp, const 
     if (!net || !smp || smp->n < 0 || !grad_enc) return NGP_EINVAL;
     if (smp->n == 0) return 0;
     if (!dL_dh || !feat_save || !workspace || workspace_bytes < ngp_net_backward_workspace(smp->n)) return NGP_EINVAL;
-    static bool attr = false;
-    if (!attr) {
-        NGP_CUDA(cudaFuncSetAttribute(k_enc_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncBwdSmem)));
-        attr = true;
-    }
+    NGP_CUDA(ngp_smem_opt_in<k_enc_bwd>((int)sizeof(EncBwdSmem)));
     const int64_t n_mtiles = (smp->n + 15) / 16;
     const int64_t n_blks = (n_mtiles + MOD_WARPS - 1) / MOD_WARPS;
     const int grid = (int)(n_blks < (int64_t)ngp_sm_count() ? n_blks : ngp_sm_count());

@@ -4,8 +4,7 @@
 // vector reductions. Replaces the three tinycudann modules of reference models/networks.py:36-77 and
 // the glue of NGP.density / NGP.forward (networks.py:94-107, :132-153).
 #include "common.cuh"
-#include "hashgrid.cuh"
-#include "mlp.cuh"
+#include "network.cuh"
 #include "wgmma.cuh"
 #include "../../include/ngp_b200.h"
 #include <math.h>
@@ -153,6 +152,16 @@ __device__ __forceinline__ int64_t bwd_count(const NgpSamples& s) {
     return sample_count(s);
 }
 
+// the sample at t on ray r, with the rounding of the marcher's sample position (march.cuh: x = fma(d, t, o))
+__device__ __forceinline__ SampleIn ray_sample(const NgpSamples& s, int r, float t) {
+    SampleIn o;
+    o.dx = __ldg(s.rays_d + 3 * r); o.dy = __ldg(s.rays_d + 3 * r + 1); o.dz = __ldg(s.rays_d + 3 * r + 2);
+    o.x = __fmaf_rn(o.dx, t, __ldg(s.rays_o + 3 * r));
+    o.y = __fmaf_rn(o.dy, t, __ldg(s.rays_o + 3 * r + 1));
+    o.z = __fmaf_rn(o.dz, t, __ldg(s.rays_o + 3 * r + 2));
+    return o;
+}
+
 __device__ __forceinline__ SampleIn load_sample(const NgpSamples& s, int64_t i, bool& valid) {
     SampleIn o;
     if (!valid) {
@@ -168,12 +177,7 @@ __device__ __forceinline__ SampleIn load_sample(const NgpSamples& s, int64_t i, 
             o.dx = 0.f; o.dy = 0.f; o.dz = 1.f;
             return o;
         }
-        const float t = __ldg(s.ts + i);
-        o.dx = __ldg(s.rays_d + 3 * r); o.dy = __ldg(s.rays_d + 3 * r + 1); o.dz = __ldg(s.rays_d + 3 * r + 2);
-        // same rounding as the marcher's sample position (march.cuh: x = fma(d, t, o))
-        o.x = __fmaf_rn(o.dx, t, __ldg(s.rays_o + 3 * r));
-        o.y = __fmaf_rn(o.dy, t, __ldg(s.rays_o + 3 * r + 1));
-        o.z = __fmaf_rn(o.dz, t, __ldg(s.rays_o + 3 * r + 2));
+        o = ray_sample(s, r, __ldg(s.ts + i));
     } else {
         o.x = __ldg(s.xyzs + 3 * i); o.y = __ldg(s.xyzs + 3 * i + 1); o.z = __ldg(s.xyzs + 3 * i + 2);
         if (s.dirs) {
@@ -185,8 +189,22 @@ __device__ __forceinline__ SampleIn load_sample(const NgpSamples& s, int64_t i, 
     return o;
 }
 
-__device__ __forceinline__ float sel4(int q, float a, float b, float c, float d) {
-    return q == 0 ? a : (q == 1 ? b : (q == 2 ? c : d));
+// a point of a lattice, generated from its row-major index: x = lo + (float)i * step, an fp32 multiply then an fp32 add,
+// so the points are bitwise those a caller materialises with the same formula
+__device__ __forceinline__ int64_t sample_count(const NgpLattice& lat) { return (int64_t)lat.n[0] * lat.n[1] * lat.n[2]; }
+__device__ __forceinline__ SampleIn load_sample(const NgpLattice& lat, int64_t row, bool& valid) {
+    SampleIn s;
+    s.x = s.y = s.z = 0.f;
+    s.dx = 0.f; s.dy = 0.f; s.dz = 1.f;
+    if (valid) {
+        const int64_t n1 = lat.n[1], n2 = lat.n[2];
+        const int64_t k = row % n2, ij = row / n2;
+        const int64_t j = ij % n1, i = ij / n1;
+        s.x = __fadd_rn(lat.lo[0], __fmul_rn((float)i, lat.step[0]));
+        s.y = __fadd_rn(lat.lo[1], __fmul_rn((float)j, lat.step[1]));
+        s.z = __fadd_rn(lat.lo[2], __fmul_rn((float)k, lat.step[2]));
+    }
+    return s;
 }
 
 // x01 = (x - xyz_min) / (xyz_max - xyz_min)   (reference networks.py:103)
@@ -216,27 +234,16 @@ __device__ __forceinline__ void encode_rows(const NgpNet& net, const uint32_t* _
             }
 }
 
-// SH-4 of the normalised direction, as the A fragment k-tile 0 of the rgb net input.
-__device__ __forceinline__ void sh_rows(const SampleIn& s, int q, uint32_t& lo, uint32_t& hi) {
-    const float inv = 1.0f / sqrtf(s.dx * s.dx + s.dy * s.dy + s.dz * s.dz);
-    float sh[16];
-    sh4(s.dx * inv, s.dy * inv, s.dz * inv, sh);
-    lo = pack_half2(sel4(q, sh[0], sh[2], sh[4], sh[6]), sel4(q, sh[1], sh[3], sh[5], sh[7]));
-    hi = pack_half2(sel4(q, sh[8], sh[10], sh[12], sh[14]), sel4(q, sh[9], sh[11], sh[13], sh[15]));
-}
-
-__device__ __forceinline__ float half_round(float v) { return __half2float(__float2half_rn(v)); }
-__device__ __forceinline__ float lo_half(uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u & 0xffffu))); }
-__device__ __forceinline__ float hi_half(uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u >> 16))); }
-
 // -------------------------------------------------------------------------------------------------
-// forward
+// forward. Rows: the samples of an NgpSamples, or the points of an NgpLattice generated from the row index (mesh
+// extraction, ngp_pl_b200/mesh.py: density only, 4 B a point written).
 // -------------------------------------------------------------------------------------------------
 #define FWD_MT 1            // 16-row tiles a warp takes at a time
 #define FWD_THREADS 256
 #define FWD_MIN_BLOCKS 3    // CTAs per SM: 24 warps
+template <typename Rows>
 __global__ void __launch_bounds__(FWD_THREADS, FWD_MIN_BLOCKS)
-k_ngp_fwd(const NgpNet net, const NgpSamples smp, const int want_rgb, float* __restrict__ sigmas, float* __restrict__ rgbs,
+k_ngp_fwd(const NgpNet net, const Rows smp, const int want_rgb, float* __restrict__ sigmas, float* __restrict__ rgbs,
           __half* __restrict__ h_out, uint4* __restrict__ feat_save, int* __restrict__ sched) {
     __shared__ __align__(16) MlpWeightsFwd sw;
     // (eager callers may write the weights or the samples with the kernel right before this one: wait first)
@@ -285,27 +292,15 @@ k_ngp_fwd(const NgpNet net, const NgpSamples smp, const int want_rgb, float* __r
                         make_uint4(featA[mt][kt][0], featA[mt][kt][1], featA[mt][kt][2], featA[mt][kt][3]);
         }
 
-        // density MLP: 32 -> 64 (ReLU) -> 16
-        uint32_t hidA[FWD_MT][4][4];
-        {
-            float hidC[FWD_MT][8][4];
-            mlp_layer<FWD_MT, 32, 64, LD32>(featA, sw.w1d, hidC, g, q);
-            relu_to_frag<FWD_MT, 64>(hidC, hidA);
-        }
         uint32_t hA[FWD_MT][1][4];
-        {
-            float hC[FWD_MT][2][4];
-            mlp_layer<FWD_MT, 64, 16, LD64>(hidA, sw.w2d, hC, g, q);
-            to_frag<FWD_MT, 16>(hC, hA);  // tinycudann returns fp16
-        }
+        density_mlp<FWD_MT>(featA, sw.w1d, sw.w2d, hA, g, q, [](const auto&) {});
 #pragma unroll
         for (int mt = 0; mt < FWD_MT; ++mt)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int64_t row = base + 16 * mt + g + 8 * h;
                 if (valid[mt][h]) {
-                    // sigma = exp(h[:,0]) in fp32 (reference networks.py:105, custom_functions.py:162-167)
-                    if (q == 0) sigmas[row] = expf(lo_half(hA[mt][0][h]));
+                    if (q == 0) sigmas[row] = sigma_of_h(hA[mt][0][h]);
                     if (h_out) {
                         uint32_t* ho = reinterpret_cast<uint32_t*>(h_out + row * 16);
                         ho[q] = hA[mt][0][h];
@@ -315,51 +310,33 @@ k_ngp_fwd(const NgpNet net, const NgpSamples smp, const int want_rgb, float* __r
             }
         if (!want_rgb) continue;
 
-        // rgb MLP input: [SH16(dir) | h16]
         uint32_t inA[FWD_MT][2][4];
-#pragma unroll
-        for (int mt = 0; mt < FWD_MT; ++mt) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) sh_rows(sm[mt][h], q, inA[mt][0][h], inA[mt][0][2 + h]);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) inA[mt][1][e] = hA[mt][0][e];
-        }
-        uint32_t r1A[FWD_MT][4][4];
-        {
-            float c[FWD_MT][8][4];
-            mlp_layer<FWD_MT, 32, 64, LD32>(inA, sw.w1r, c, g, q);
-            relu_to_frag<FWD_MT, 64>(c, r1A);
-        }
-        uint32_t r2A[FWD_MT][4][4];
-        {
-            float c[FWD_MT][8][4];
-            mlp_layer<FWD_MT, 64, 64, LD64>(r1A, sw.w2r, c, g, q);
-            relu_to_frag<FWD_MT, 64>(c, r2A);
-        }
+        color_input<FWD_MT>(sm, hA, q, inA);
         float oC[FWD_MT][1][4];
-        mlp_layer<FWD_MT, 64, 8, LD64>(r2A, sw.w3r, oC, g, q);  // only output columns 0..7 are needed (rgb = 0..2)
+        color_mlp<FWD_MT>(inA, sw.w1r, sw.w2r, sw.w3r, oC, g, q, [](int, const auto&) {});
 #pragma unroll
         for (int mt = 0; mt < FWD_MT; ++mt)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int64_t row = base + 16 * mt + g + 8 * h;
                 if (!valid[mt][h] || q > 1) continue;
-                float a = oC[mt][0][2 * h], b = oC[mt][0][2 * h + 1];
-                if (net.rgb_act == 1) {
-                    a = 1.0f / (1.0f + __expf(-a));
-                    b = 1.0f / (1.0f + __expf(-b));
-                }
-                a = half_round(a);
-                b = half_round(b);
+                const float2 o = __half22float2(rgb_out(oC[mt][0][2 * h], oC[mt][0][2 * h + 1], net.rgb_act));
                 if (q == 0) {
-                    rgbs[3 * row] = a;
-                    rgbs[3 * row + 1] = b;
+                    rgbs[3 * row] = o.x;
+                    rgbs[3 * row + 1] = o.y;
                 } else {
-                    rgbs[3 * row + 2] = a;
+                    rgbs[3 * row + 2] = o.x;
                 }
             }
     }
     sched_finish(sched);
+}
+
+static int fwd_grid(int64_t n) {
+    const int64_t n_tiles = (n + 16 * FWD_MT - 1) / (16 * FWD_MT);
+    const int64_t want = (n_tiles + FWD_THREADS / 32 - 1) / (FWD_THREADS / 32);
+    const int64_t cap = (int64_t)ngp_sm_count() * FWD_MIN_BLOCKS;
+    return (int)(want < cap ? want : cap);
 }
 
 extern "C" int ngp_net_forward(const NgpNet* net, const NgpSamples* smp, int want_rgb, float* sigmas, float* rgbs,
@@ -368,83 +345,22 @@ extern "C" int ngp_net_forward(const NgpNet* net, const NgpSamples* smp, int wan
     if (net->meta.n_levels < 1 || net->meta.n_levels > NGP_MAX_LEVELS) return NGP_EINVAL;
     if (smp->n == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    const int64_t n_tiles = (smp->n + 16 * FWD_MT - 1) / (16 * FWD_MT);
-    const int64_t want = (n_tiles + FWD_THREADS / 32 - 1) / (FWD_THREADS / 32);
-    const int64_t cap = (int64_t)ngp_sm_count() * FWD_MIN_BLOCKS;
-    const int grid = (int)(want < cap ? want : cap);
-    NGP_CUDA(ngp_launch_pdl(k_ngp_fwd, grid, FWD_THREADS, 0, st, *net, *smp, want_rgb, sigmas, rgbs, (__half*)h_out,
-                            (uint4*)feat_save, sched_slot(st)));
+    NGP_CUDA(ngp_launch_pdl(k_ngp_fwd<NgpSamples>, fwd_grid(smp->n), FWD_THREADS, 0, st, *net, *smp, want_rgb, sigmas, rgbs,
+                            (__half*)h_out, (uint4*)feat_save, sched_slot(st)));
     NGP_CHECK_LAUNCH();
     NGP_TRACE(3, st);
     return 0;
 }
 
-// -------------------------------------------------------------------------------------------------
-// density on a lattice (mesh extraction, ngp_pl_b200/mesh.py): k_ngp_fwd's density-only path with the rows generated
-// from the tile index instead of read -- x = lo + (float)idx * step, an fp32 multiply then an fp32 add, so the points
-// are bitwise those a caller materialises with the same formula -- and only sigma written (4 B a point).
-// -------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(FWD_THREADS, FWD_MIN_BLOCKS)
-k_density_lattice(const NgpNet net, const NgpLattice lat, float* __restrict__ sigma) {
-    __shared__ __align__(16) MlpWeightsFwd sw;
-    const __half* wd = reinterpret_cast<const __half*>(net.enc_params_h);
-    load_weights_fwd(sw, wd, nullptr, threadIdx.x, FWD_THREADS);
-    __syncthreads();
-    const uint32_t* table = reinterpret_cast<const uint32_t*>(wd + NGP_DENSITY_MLP_PARAMS);
-
-    const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
-    const int64_t n1 = lat.n[1], n2 = lat.n[2];
-    const int64_t n = (int64_t)lat.n[0] * n1 * n2;
-    const int64_t n_tiles = (n + 15) / 16;
-    const int64_t n_warps = (int64_t)gridDim.x * (FWD_THREADS / 32);
-    for (int64_t tile = (int64_t)blockIdx.x * (FWD_THREADS / 32) + (threadIdx.x >> 5); tile < n_tiles; tile += n_warps) {
-        bool valid[1][2];
-        float u[1][2][3];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int64_t row = tile * 16 + g + 8 * h;
-            valid[0][h] = row < n;
-            SampleIn s;
-            s.x = s.y = s.z = 0.f;
-            s.dx = 0.f; s.dy = 0.f; s.dz = 1.f;
-            if (valid[0][h]) {
-                const int64_t k = row % n2, ij = row / n2;
-                const int64_t j = ij % n1, i = ij / n1;
-                s.x = __fadd_rn(lat.lo[0], __fmul_rn((float)i, lat.step[0]));
-                s.y = __fadd_rn(lat.lo[1], __fmul_rn((float)j, lat.step[1]));
-                s.z = __fadd_rn(lat.lo[2], __fmul_rn((float)k, lat.step[2]));
-            }
-            to_unit(net, s, u[0][h][0], u[0][h][1], u[0][h][2]);
-        }
-        uint32_t featA[1][2][4];
-        encode_rows<1>(net, table, u, valid, featA, q);
-        uint32_t hidA[1][4][4];
-        {
-            float hidC[1][8][4];
-            mlp_layer<1, 32, 64, LD32>(featA, sw.w1d, hidC, g, q);
-            relu_to_frag<1, 64>(hidC, hidA);
-        }
-        uint32_t hA[1][1][4];
-        {
-            float hC[1][2][4];
-            mlp_layer<1, 64, 16, LD64>(hidA, sw.w2d, hC, g, q);
-            to_frag<1, 16>(hC, hA);
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-            if (valid[0][h] && q == 0) sigma[tile * 16 + g + 8 * h] = expf(lo_half(hA[0][0][h]));
-    }
-}
-
+// density on a lattice: static striding (no scheduler slot), sigma only
 extern "C" int ngp_density_lattice(const NgpNet* net, const NgpLattice* lat, float* sigma, void* stream) {
     if (!net || !lat || !sigma || !net->enc_params_h) return NGP_EINVAL;
     if (net->meta.n_levels < 1 || net->meta.n_levels > NGP_MAX_LEVELS) return NGP_EINVAL;
     for (int a = 0; a < 3; ++a)
         if (lat->n[a] < 2) return NGP_EINVAL;
     const int64_t n = (int64_t)lat->n[0] * lat->n[1] * lat->n[2];
-    const int64_t want = ((n + 15) / 16 + FWD_THREADS / 32 - 1) / (FWD_THREADS / 32);
-    const int64_t cap = (int64_t)ngp_sm_count() * FWD_MIN_BLOCKS;
-    k_density_lattice<<<(int)(want < cap ? want : cap), FWD_THREADS, 0, (cudaStream_t)stream>>>(*net, *lat, sigma);
+    k_ngp_fwd<NgpLattice><<<fwd_grid(n), FWD_THREADS, 0, (cudaStream_t)stream>>>(*net, *lat, 0, sigma, nullptr, nullptr, nullptr,
+                                                                                  nullptr);
     NGP_CHECK_LAUNCH();
     return 0;
 }
@@ -701,7 +617,7 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
         const int64_t base = mtile * 16;
         bool valid[2];
         float up_sig[2], up_c0[2], up_c1[2];
-        SampleIn sm[2];
+        SampleIn sm[1][2];
         uint32_t featA[1][2][4];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -713,15 +629,10 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
                 featA[0][kt][2 + h] = pre_feat[kt][2 + h];
             }
             if (valid[h] && pre_ridx[h] >= 0) {
-                const int r = pre_ridx[h];
-                const float t = pre_t[h];
-                sm[h].dx = __ldg(smp.rays_d + 3 * r); sm[h].dy = __ldg(smp.rays_d + 3 * r + 1); sm[h].dz = __ldg(smp.rays_d + 3 * r + 2);
-                sm[h].x = __fmaf_rn(sm[h].dx, t, __ldg(smp.rays_o + 3 * r));
-                sm[h].y = __fmaf_rn(sm[h].dy, t, __ldg(smp.rays_o + 3 * r + 1));
-                sm[h].z = __fmaf_rn(sm[h].dz, t, __ldg(smp.rays_o + 3 * r + 2));
+                sm[0][h] = ray_sample(smp, pre_ridx[h], pre_t[h]);
             } else {
                 bool v = valid[h];
-                sm[h] = load_sample(smp, pre_src[h], v);  // (xyzs / dirs layout, or an invalid row)
+                sm[0][h] = load_sample(smp, pre_src[h], v);  // (xyzs / dirs layout, or an invalid row)
                 valid[h] = v;
             }
         }
@@ -730,7 +641,7 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
             const bool v[1][2] = {{valid[0], valid[1]}};
             float u[1][2][3];
 #pragma unroll
-            for (int h = 0; h < 2; ++h) to_unit(net, sm[h], u[0][h][0], u[0][h][1], u[0][h][2]);
+            for (int h = 0; h < 2; ++h) to_unit(net, sm[0][h], u[0][h][0], u[0][h][1], u[0][h][2]);
             encode_rows<1>(net, table, u, v, featA, q);
         }
         // the previous block's GEMMs still read feat / hid / rin / r1 / r2: its last batch (W1d, buffer 0) completes after
@@ -745,58 +656,26 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
         stage_canon<2>(S.feat, 32, row0, featA[0], g, q);
         float h0[2];
         uint32_t hA[1][1][4];
-        {
-            uint32_t hidA[1][4][4];
-            {
-                float c[1][8][4];
-                mlp_layer<1, 32, 64, LD32>(featA, S.wf.w1d, c, g, q);
-                relu_to_frag<1, 64>(c, hidA);
-            }
-            stage_canon<4>(S.hid, 64, row0, hidA[0], g, q);
-            float c[1][2][4];
-            mlp_layer<1, 64, 16, LD64>(hidA, S.wf.w2d, c, g, q);
-            to_frag<1, 16>(c, hA);
-        }
+        density_mlp<1>(featA, S.wf.w1d, S.wf.w2d, hA, g, q,
+                       [&](const auto& hid) { stage_canon<4>(S.hid, 64, row0, hid[0], g, q); });
         h0[0] = lo_half(hA[0][0][0]);
         h0[1] = lo_half(hA[0][0][1]);
         uint32_t doutA[1][1][4];
         {
             uint32_t inA[1][2][4];
-#pragma unroll
-            for (int h = 0; h < 2; ++h) sh_rows(sm[h], q, inA[0][0][h], inA[0][0][2 + h]);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) inA[0][1][e] = hA[0][0][e];
+            color_input<1>(sm, hA, q, inA);
             stage_canon<2>(S.rin, 32, row0, inA[0], g, q);
-            uint32_t r1A[1][4][4];
-            {
-                float c[1][8][4];
-                mlp_layer<1, 32, 64, LD32>(inA, S.wf.w1r, c, g, q);
-                relu_to_frag<1, 64>(c, r1A);
-            }
-            stage_canon<4>(S.r1, 64, row0, r1A[0], g, q);
-            uint32_t r2A[1][4][4];
-            {
-                float c[1][8][4];
-                mlp_layer<1, 64, 64, LD64>(r1A, S.wf.w2r, c, g, q);
-                relu_to_frag<1, 64>(c, r2A);
-            }
-            stage_canon<4>(S.r2, 64, row0, r2A[0], g, q);
             float oC[1][1][4];
-            mlp_layer<1, 64, 8, LD64>(r2A, S.wf.w3r, oC, g, q);
+            color_mlp<1>(inA, S.wf.w1r, S.wf.w2r, S.wf.w3r, oC, g, q,
+                         [&](int l, const auto& r) { stage_canon<4>(l == 1 ? S.r1 : S.r2, 64, row0, r[0], g, q); });
             doutA[0][0][2] = 0u;
             doutA[0][0][3] = 0u;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 float d0 = 0.f, d1 = 0.f;
                 if (valid[h] && q < 2) {
-                    float o0 = oC[0][0][2 * h], o1 = oC[0][0][2 * h + 1];
-                    float s0 = 1.f, s1 = 1.f;
-                    if (net.rgb_act == 1) {
-                        o0 = half_round(1.0f / (1.0f + __expf(-o0)));
-                        o1 = half_round(1.0f / (1.0f + __expf(-o1)));
-                        s0 = o0 * (1.0f - o0);
-                        s1 = o1 * (1.0f - o1);
-                    }
+                    float s0 = oC[0][0][2 * h], s1 = oC[0][0][2 * h + 1];
+                    rgb_out_grad(s0, s1, net.rgb_act);
                     d0 = up_c0[h] * s0 * scale;
                     d1 = (q == 0) ? up_c1[h] * s1 * scale : 0.f;
                 }
@@ -1010,17 +889,8 @@ extern "C" int ngp_net_backward_mlp(const NgpNet* net, const NgpSamples* smp, co
     if (!dL_dsigmas || !dL_drgbs || !grad_enc || !grad_rgb) return NGP_EINVAL;
     if (smp->live_idx && (!smp->n_live_dev || !feat_save)) return NGP_EINVAL;  // a live list needs the saved features
     if (smp->n == 0) return 0;
-    {
-        // the dynamic shared-memory opt-in is a per-DEVICE function attribute: one process may drive several GPUs
-        static unsigned char attr_set[64] = {0};
-        int dev = 0;
-        NGP_CUDA(cudaGetDevice(&dev));
-        if (dev < 0 || dev >= 64 || !__atomic_load_n(&attr_set[dev], __ATOMIC_ACQUIRE)) {
-            NGP_CUDA(cudaFuncSetAttribute(k_ngp_bwd3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Bwd3Smem) + 128));
-            NGP_CUDA(cudaFuncSetAttribute(k_ngp_bwd3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Bwd3Smem) + 128));
-            if (dev >= 0 && dev < 64) __atomic_store_n(&attr_set[dev], 1, __ATOMIC_RELEASE);
-        }
-    }
+    const int smem = (int)sizeof(Bwd3Smem) + 128;
+    NGP_CUDA(feat_save ? ngp_smem_opt_in<k_ngp_bwd3<false>>(smem) : ngp_smem_opt_in<k_ngp_bwd3<true>>(smem));
     const int64_t n_mtiles = (smp->n + 15) / 16;
     const int64_t n_blks = (n_mtiles + B3_WARPS - 1) / B3_WARPS;
     const int grid = (int)(n_blks < (int64_t)ngp_sm_count() ? n_blks : ngp_sm_count());
