@@ -303,7 +303,10 @@ int ngp_nerf_loss_grad(const NgpTrainCfg* cfg, const NgpTrainBuffers* buf, const
 
 /* Fused Adam over a flat fp32 vector (apex FusedAdam semantics as the reference uses it, train.py:131:
  * adam_w_mode, weight_decay 0, bias correction, eps): p -= lr * m_hat / (sqrt(v_hat) + eps), with
- * g = grads * grad_mul (1/world_size after a sum all-reduce). Also refreshes the fp16 working copy and
+ * g = grads * grad_mul (1/world_size after a sum all-reduce). The bias corrections are apex's: 1 - beta^t computed in
+ * double and rounded to float once (in float, 1 - powf(0.999, t) loses ~100 roundings to cancellation at small t).
+ * ngp_adam_step_p2p / _fused share this update: on the same inputs they agree with it bit for bit. Also refreshes
+ * the fp16 working copy and
  * zeroes the gradient for the next step in the same pass. lr and step live on the device
  * (lr_dev[0], step_dev[0] = number of completed steps; the kernel uses t = step+1 and a follow-up
  * single-thread kernel increments it) so a captured CUDA graph never needs re-capturing. Launched as a programmatic

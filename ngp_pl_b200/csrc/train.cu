@@ -456,17 +456,43 @@ extern "C" int ngp_nerf_loss_grad(const NgpTrainCfg* cfg, const NgpTrainBuffers*
 }
 
 // -------------------------------------------------------------------------------------------------
+// The Adam core of every optimiser kernel (k_adam, k_adam_p2p, k_adam_fused): the per-step constants and the update of
+// one element, written once with explicit roundings so that the kernels agree bit for bit by construction.
+// -------------------------------------------------------------------------------------------------
+struct AdamConsts {
+    float beta1, beta2, eps, grad_mul, step_size, inv_sqrt_bc2;
+};
+// t = *step_dev + 1. The bias corrections are apex FusedAdam's: 1 - beta^t in double, rounded to float once. In float,
+// 1 - powf(beta2, t) cancels at small t (beta2 = 0.999) and loses up to ~100 float roundings of bc2.
+__device__ __forceinline__ AdamConsts adam_consts(const float* lr_dev, const int* step_dev, float beta1, float beta2,
+                                                  float eps, float grad_mul) {
+    const double t = (double)(*step_dev + 1);
+    const float bc1 = (float)(1.0 - pow((double)beta1, t));
+    const float bc2 = (float)(1.0 - pow((double)beta2, t));
+    return AdamConsts{beta1, beta2, eps, grad_mul, __fdiv_rn(*lr_dev, bc1), rsqrtf(bc2)};
+}
+// p -= step_size * m' / (sqrt(v') * inv_sqrt_bc2 + eps) with m' = beta1 m + (1 - beta1) g, v' = beta2 v + (1 - beta2) g^2
+__device__ __forceinline__ void adam_update(const AdamConsts& c, float& p, const float g, float& m, float& v) {
+    const float gr = __fmul_rn(g, c.grad_mul);
+    m = __fmaf_rn(c.beta1, m, __fmul_rn(1.0f - c.beta1, gr));
+    v = __fmaf_rn(c.beta2, v, __fmul_rn(__fmul_rn(1.0f - c.beta2, gr), gr));
+    const float denom = __fmaf_rn(__fsqrt_rn(v), c.inv_sqrt_bc2, c.eps);
+    p = __fmaf_rn(-c.step_size, __fdiv_rn(m, denom), p);
+}
+__device__ __forceinline__ void adam_update4(const AdamConsts& c, float4& p, const float4 g, float4& m, float4& v) {
+    adam_update(c, p.x, g.x, m.x, v.x);
+    adam_update(c, p.y, g.y, m.y, v.y);
+    adam_update(c, p.z, g.z, m.z, v.z);
+    adam_update(c, p.w, g.w, m.w, v.w);
+}
+
+// -------------------------------------------------------------------------------------------------
 // fused Adam (+ fp16 re-cast + gradient zeroing), 128-bit accesses
 // -------------------------------------------------------------------------------------------------
 __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                        __half* __restrict__ ph, int64_t n, const float* __restrict__ lr_dev, const int* __restrict__ step_dev,
                        float beta1, float beta2, float eps, float grad_mul) {
-    const int t = *step_dev + 1;
-    const float lr = *lr_dev;
-    const float bc1 = 1.0f - powf(beta1, (float)t);
-    const float bc2 = 1.0f - powf(beta2, (float)t);
-    const float step_size = lr / bc1;
-    const float inv_sqrt_bc2 = rsqrtf(bc2);
+    const AdamConsts c = adam_consts(lr_dev, step_dev, beta1, beta2, eps, grad_mul);
     const int64_t n4 = n >> 2;
     // fp32 params, moments and the consumed gradients stream through L2 (evict first); the fp16 working copy the
     // forward gathers from is kept (evict last); the zeroed gradients (next step's reduction target) stay normal
@@ -502,7 +528,7 @@ __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __re
         for (int u = 0; u < 2; ++u) {
             if (u == 1 && !two) break;
             const int64_t i = u ? i1 : i0;
-            float* pp = &pv[u].x; float* gp = &gv[u].x; float* mp = &mv[u].x; float* vp = &vv[u].x;
+            const float* gp = &gv[u].x; const float* mp = &mv[u].x; const float* vp = &vv[u].x;
             // Stores that cannot change memory are skipped (bitwise the same result, 18 of the 34 bytes per parameter):
             // a hash-table entry no ray has touched yet has g = m = v = 0, its update is p -= lr * 0 / (0 + eps);
             // and a gradient that already is zero needs no clearing. Most of the fine levels' entries are in one of the
@@ -511,14 +537,7 @@ __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __re
             if (g_zero && mp[0] == 0.f && mp[1] == 0.f && mp[2] == 0.f && mp[3] == 0.f && vp[0] == 0.f && vp[1] == 0.f &&
                 vp[2] == 0.f && vp[3] == 0.f)
                 continue;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const float gr = gp[k] * grad_mul;
-                mp[k] = beta1 * mp[k] + (1.0f - beta1) * gr;
-                vp[k] = beta2 * vp[k] + (1.0f - beta2) * gr * gr;
-                const float denom = sqrtf(vp[k]) * inv_sqrt_bc2 + eps;
-                pp[k] -= step_size * (mp[k] / denom);
-            }
+            adam_update4(c, pv[u], gv[u], mv[u], vv[u]);
             st_f4_hint(reinterpret_cast<float4*>(p) + i, pv[u], stream_pol);
             st_f4_hint(reinterpret_cast<float4*>(m) + i, mv[u], stream_pol);
             st_f4_hint(reinterpret_cast<float4*>(v) + i, vv[u], stream_pol);
@@ -537,12 +556,13 @@ __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __re
     }
     // tail
     for (int64_t i = (n4 << 2) + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const float gr = g[i] * grad_mul;
-        m[i] = beta1 * m[i] + (1.0f - beta1) * gr;
-        v[i] = beta2 * v[i] + (1.0f - beta2) * gr * gr;
-        p[i] -= step_size * (m[i] / (sqrtf(v[i]) * inv_sqrt_bc2 + eps));
+        float pi = p[i], mi = m[i], vi = v[i];
+        adam_update(c, pi, g[i], mi, vi);
+        p[i] = pi;
+        m[i] = mi;
+        v[i] = vi;
         g[i] = 0.f;
-        if (ph) ph[i] = __float2half_rn(p[i]);
+        if (ph) ph[i] = __float2half_rn(pi);
     }
 }
 __global__ void k_step_inc(int* step) {
@@ -638,12 +658,7 @@ struct PeerPtrs {
 __global__ void k_adam_p2p(const PeerPtrs peers, const int world, float* __restrict__ p, float* __restrict__ m,
                            float* __restrict__ v, const int64_t lo4, const int64_t hi4, const float* __restrict__ lr_dev,
                            const int* __restrict__ step_dev, float beta1, float beta2, float eps, float grad_mul) {
-    const int t = *step_dev + 1;
-    const float lr = *lr_dev;
-    const float bc1 = 1.0f - powf(beta1, (float)t);
-    const float bc2 = 1.0f - powf(beta2, (float)t);
-    const float step_size = lr / bc1;
-    const float inv_sqrt_bc2 = rsqrtf(bc2);
+    const AdamConsts c = adam_consts(lr_dev, step_dev, beta1, beta2, eps, grad_mul);
     const uint64_t stream_pol = l2_policy_evict_first();
     for (int64_t i = lo4 + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < hi4; i += (int64_t)gridDim.x * blockDim.x) {
         float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -657,14 +672,7 @@ __global__ void k_adam_p2p(const PeerPtrs peers, const int world, float* __restr
         float4 pv = ld_f4_hint(reinterpret_cast<const float4*>(p) + i, stream_pol);
         float4 mv = ld_f4_hint(reinterpret_cast<const float4*>(m) + i, stream_pol);
         float4 vv = ld_f4_hint(reinterpret_cast<const float4*>(v) + i, stream_pol);
-        float* pp = &pv.x; float* gp = &g.x; float* mp = &mv.x; float* vp = &vv.x;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const float gr = gp[k] * grad_mul;
-            mp[k] = beta1 * mp[k] + (1.0f - beta1) * gr;
-            vp[k] = beta2 * vp[k] + (1.0f - beta2) * gr * gr;
-            pp[k] -= step_size * (mp[k] / (sqrtf(vp[k]) * inv_sqrt_bc2 + eps));
-        }
+        adam_update4(c, pv, g, mv, vv);
         st_f4_hint(reinterpret_cast<float4*>(p) + i, pv, stream_pol);
         st_f4_hint(reinterpret_cast<float4*>(m) + i, mv, stream_pol);
         st_f4_hint(reinterpret_cast<float4*>(v) + i, vv, stream_pol);
@@ -805,12 +813,7 @@ k_adam_fused(const FusedPeers peers, const int world, const int rank, float* __r
         if (threadIdx.x == 0 && !wait_epoch<false>(&sync[3], e)) sync[2] = 1u;
         __syncthreads();
     }
-    const int t = *step_dev + 1;
-    const float lr = *lr_dev;
-    const float bc1 = 1.0f - powf(beta1, (float)t);
-    const float bc2 = 1.0f - powf(beta2, (float)t);
-    const float step_size = lr / bc1;
-    const float inv_sqrt_bc2 = rsqrtf(bc2);
+    const AdamConsts c = adam_consts(lr_dev, step_dev, beta1, beta2, eps, grad_mul);
     const uint64_t stream_pol = l2_policy_evict_first();
     const bool mc_in = peers.mc_grads != nullptr, mc_out = peers.mc_params_half != nullptr;
     // U float4 groups per thread per trip, their remote loads issued back to back before anything waits on them: one
@@ -823,18 +826,12 @@ k_adam_fused(const FusedPeers peers, const int world, const int rank, float* __r
         float4 pv = ld_f4_hint(reinterpret_cast<const float4*>(p) + i, stream_pol);
         float4 mv = ld_f4_hint(reinterpret_cast<const float4*>(m) + i, stream_pol);
         float4 vv = ld_f4_hint(reinterpret_cast<const float4*>(v) + i, stream_pol);
-        float* pp = &pv.x; float* gp = &g.x; float* mp = &mv.x; float* vp = &vv.x;
+        const float* gp = &g.x; const float* mp = &mv.x; const float* vp = &vv.x;
         // untouched entries (g = m = v = 0 on every rank): nothing changes, nothing to store or to send (see k_adam)
         if (gp[0] == 0.f && gp[1] == 0.f && gp[2] == 0.f && gp[3] == 0.f && mp[0] == 0.f && mp[1] == 0.f && mp[2] == 0.f &&
             mp[3] == 0.f && vp[0] == 0.f && vp[1] == 0.f && vp[2] == 0.f && vp[3] == 0.f)
             return;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const float gr = gp[k] * grad_mul;
-            mp[k] = beta1 * mp[k] + (1.0f - beta1) * gr;
-            vp[k] = beta2 * vp[k] + (1.0f - beta2) * gr * gr;
-            pp[k] -= step_size * (mp[k] / (sqrtf(vp[k]) * inv_sqrt_bc2 + eps));
-        }
+        adam_update4(c, pv, g, mv, vv);
         st_f4_hint(reinterpret_cast<float4*>(p) + i, pv, stream_pol);
         st_f4_hint(reinterpret_cast<float4*>(m) + i, mv, stream_pol);
         st_f4_hint(reinterpret_cast<float4*>(v) + i, vv, stream_pol);
