@@ -602,6 +602,45 @@ size_t ngp_png_capacity(int H, int W);
 int ngp_png_encode(const uint8_t* img, int H, int W, uint8_t* out, size_t out_capacity, int64_t* out_len,
                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* The same file in a chosen deflate mode: NGP_PNG_FIXED is ngp_png_encode's stream byte for byte (and its workspace);
+ * NGP_PNG_DYNAMIC is a smaller stream of the same image, fixed by this algorithm (oracle/png_dynamic_ref.py restates it
+ * byte for byte):
+ *   - Filters and their Adler-32 parts: as ngp_png_encode. L = 3W + 1.
+ *   - Match search, each row on its own: the candidate distances are the distinct values of 1, 2, 3, 4, 6, 9, 12, L-3,
+ *     L, L+3 and 2L that lie in 1..32768, a candidate dropped at a position p < d. The match length for d at p is the
+ *     number of bytes s[p+i] == s[p-d+i], at most 258 and never past the row's end; the longest wins, a tie to the
+ *     smaller distance; best(p) is that length when it is >= 3, else 0 (best = 0 past the row's end).
+ *   - Lazy parse by one step from the row's first byte: at p, when best(p) >= 3 and best(p+1) <= best(p), the match
+ *     (best(p), its distance) is emitted and the parse skips it; otherwise the byte is a literal and the parse moves on
+ *     by one. Tokens are coded with RFC 1951's length and distance codes and extra bits.
+ *   - Groups: rows 32g .. 32g + 31 (the last group shorter) form one block, their tokens concatenated bit by bit, then
+ *     end-of-block. Histograms: the group's literal/length symbols plus one end-of-block, and its distance codes.
+ *   - Dynamic code: lengths by package-merge, limit 15 for both alphabets; items sorted by (count, symbol) ascending,
+ *     an item before a package of equal weight; the first 2n - 2 entries of the last list give the lengths. A single
+ *     used symbol gets length 1; with no distance code used, distance code 0 gets length 1. Canonical codes (RFC 1951
+ *     3.2.2). HLIT = max(257, last used literal/length + 1), HDIST = max(1, last nonzero distance length + 1). The two
+ *     length lists are run-length coded separately by zlib's send_tree rules (16: 3-6 repeats of the previous length,
+ *     17: 3-10 zeros, 18: 11-138 zeros); the code-length code by package-merge with limit 7 over those symbols,
+ *     HCLEN = the RFC's permutation order trimmed of trailing zero lengths, at least 4.
+ *   - Each group is coded as one dynamic block (BTYPE 10), one fixed block (BTYPE 01) or stored blocks of at most 65535
+ *     bytes of the group's filtered bytes (BTYPE 00), whichever is shortest in bytes with the empty stored block that
+ *     follows it (3 header bits, padding, LEN 0000, NLEN ffff), a tie in that order; BFINAL is 0 on each, and 1 on the
+ *     last group's empty block. Every group therefore starts on a byte boundary.
+ *   - Assembly as ngp_png_encode with the groups in place of the rows: offsets from a scan of the groups' lengths, the
+ *     IDAT CRC-32 combined from per-group CRCs; the Adler-32 still from per-row parts.
+ *   - All arithmetic is integer and fixed-order: two calls give the same bytes.
+ * ngp_png_capacity bounds both modes (a group stored whole is never longer than its rows stored one by one).
+ * ngp_png_workspace_mode(H, W, NGP_PNG_DYNAMIC) covers the filtered stream, the match table (2 H L), token-start masks,
+ * per-row histograms (1264 H), row offsets, the group tables and buffers; it is 0 where ngp_png_workspace is, and for
+ * an unknown mode. ngp_png_encode_mode returns NGP_EINVAL for an unknown mode and for everything ngp_png_encode
+ * refuses. Dynamic mode: seven kernels (filter, match and parse, tables, emission, group CRCs, assembly, compaction);
+ * no synchronisation. */
+#define NGP_PNG_FIXED 0
+#define NGP_PNG_DYNAMIC 1
+size_t ngp_png_workspace_mode(int H, int W, int mode);
+int ngp_png_encode_mode(const uint8_t* img, int H, int W, int mode, uint8_t* out, size_t out_capacity, int64_t* out_len,
+                        void* workspace, size_t workspace_bytes, void* stream);
+
 /* One complete baseline JPEG of img (H, W, 3) uint8 RGB (device), for the Motion-JPEG videos of the test views. As with
  * ngp_png_encode the file goes to out and its length, an int64, to *out_len, both written by the device; out and out_len
  * may be device memory or mapped pinned host memory; nothing in the call synchronises the stream.

@@ -16,6 +16,8 @@ NGP_DENSITY_MLP_PARAMS = 3072
 NGP_RGB_MLP_PARAMS = 7168
 NGP_MC_SLAB_POINTS = 1 << 20
 NGP_VIEW_IMAGES_WORKSPACE = 4096
+NGP_PNG_FIXED = 0
+NGP_PNG_DYNAMIC = 1
 
 
 class NgpGridMeta(C.Structure):
@@ -186,6 +188,8 @@ SIGNATURES = {
     "ngp_png_workspace": (_sz, [_i, _i]),
     "ngp_png_capacity": (_sz, [_i, _i]),
     "ngp_png_encode": (_i, [_P, _i, _i, _P, _sz, _P, _P, _sz, _P]),
+    "ngp_png_workspace_mode": (_sz, [_i, _i, _i]),
+    "ngp_png_encode_mode": (_i, [_P, _i, _i, _i, _P, _sz, _P, _P, _sz, _P]),
     "ngp_jpeg_workspace": (_sz, [_i, _i]),
     "ngp_jpeg_capacity": (_sz, [_i, _i]),
     "ngp_jpeg_encode": (_i, [_P, _i, _i, _i, _P, _sz, _P, _P, _sz, _P]),

@@ -5,8 +5,11 @@ turbo depth image of a render, and PNG files of both.
     depth_image(depth, H, W) depth2img(depth) (train.py:45-50): per-view min/max, * 255, uint8, cv2's turbo colour map;
                              an (H, W, 3) uint8 device tensor whose channels are cv2's B, G, R -- the array the reference
                              writes to its `_d.png` files, blue in the red position included
-    encode_png(img)          the PNG file of an (H, W, 3) uint8 device image, as bytes
-    write_png(path, img)     the same, written to `path`
+    encode_png(img, mode="fixed")
+                             the PNG file of an (H, W, 3) uint8 device image, as bytes; mode "dynamic" writes a smaller
+                             file of the same image (dynamic Huffman blocks over a wider match search)
+    write_png(path, img, mode="fixed")
+                             the same, written to `path`
     encode_jpeg(img, quality=90), write_jpeg(path, img, quality=90)
                              the same for a baseline JPEG (4:4:4, libjpeg's bytes for that quality)
     AviWriter(path, W, H, fps)
@@ -99,39 +102,52 @@ def png_capacity(H, W):
     return n
 
 
-def png_workspace(H, W, device):
+PNG_MODES = {"fixed": _lib.NGP_PNG_FIXED, "dynamic": _lib.NGP_PNG_DYNAMIC}
+
+
+def _png_mode(mode):
+    if mode not in PNG_MODES:
+        raise ValueError("ngp_pl_b200.images: the PNG mode must be one of %s, got %r" % (sorted(PNG_MODES), mode))
+    return PNG_MODES[mode]
+
+
+def png_workspace(H, W, device, mode="fixed"):
+    m = _png_mode(mode)
     png_capacity(H, W)
-    return torch.empty(_lib.lib().ngp_png_workspace(int(H), int(W)), dtype=torch.uint8, device=device)
+    return torch.empty(_lib.lib().ngp_png_workspace_mode(int(H), int(W), m), dtype=torch.uint8, device=device)
 
 
-def encode_png_into(img, out, out_len, ws):
-    """One ngp_png_encode call on the current stream, no synchronisation: the file of img ((H, W, 3) uint8, device)
-    into out (uint8, device or pinned host memory, at least png_capacity(H, W) bytes) and its length into out_len[0]
-    (int64, device or pinned host memory). ws: png_workspace(H, W, device)."""
+def encode_png_into(img, out, out_len, ws, mode="fixed"):
+    """One ngp_png_encode_mode call on the current stream, no synchronisation: the file of img ((H, W, 3) uint8,
+    device) into out (uint8, device or pinned host memory, at least png_capacity(H, W) bytes) and its length into
+    out_len[0] (int64, device or pinned host memory). ws: png_workspace(H, W, device, mode). mode "fixed" is
+    ngp_png_encode's stream, "dynamic" the smaller one of include/ngp_b200.h."""
+    m = _png_mode(mode)
     img = _check_image(img)
     _check_buffers(out, out_len, ws)
     H, W = img.shape[0], img.shape[1]
-    rc = _lib.lib().ngp_png_encode(img.data_ptr(), H, W, out.data_ptr(), out.numel(), out_len.data_ptr(), ws.data_ptr(),
-                                   ws.numel(), _stream(img))
-    _lib.check(rc, "ngp_png_encode")
+    rc = _lib.lib().ngp_png_encode_mode(img.data_ptr(), H, W, m, out.data_ptr(), out.numel(), out_len.data_ptr(),
+                                        ws.data_ptr(), ws.numel(), _stream(img))
+    _lib.check(rc, "ngp_png_encode_mode")
 
 
 @torch.no_grad()
-def encode_png(img):
+def encode_png(img, mode="fixed"):
     """the PNG file of an (H, W, 3) uint8 device image, as bytes (written into pinned host memory by the device, so only
-    the file's bytes cross PCIe; synchronises the current stream)"""
+    the file's bytes cross PCIe; synchronises the current stream). mode: "fixed" or "dynamic" (smaller)"""
+    _png_mode(mode)
     img = _check_image(img)
     H, W = img.shape[0], img.shape[1]
     out = torch.empty(png_capacity(H, W), dtype=torch.uint8, pin_memory=True)
     n = torch.zeros(1, dtype=torch.int64, pin_memory=True)
-    encode_png_into(img, out, n, png_workspace(H, W, img.device))
+    encode_png_into(img, out, n, png_workspace(H, W, img.device, mode), mode)
     torch.cuda.current_stream(img.device).synchronize()
     return out[:int(n[0])].numpy().tobytes()
 
 
-def write_png(path, img):
+def write_png(path, img, mode="fixed"):
     """write the PNG file of an (H, W, 3) uint8 device image to path"""
-    data = encode_png(img)
+    data = encode_png(img, mode)
     with open(path, "wb") as f:
         f.write(data)
 
@@ -261,17 +277,20 @@ class ViewWriter:
 
     With video_fps, the JPEG encodes of the same two images (quality video_quality) follow the PNG encodes into the
     slot, and the writer thread appends them, in submission order, to `rgb{video_tag}.avi` and `depth{video_tag}.avi`
-    (AviWriter), finished by close(). png=False leaves the PNGs out."""
+    (AviWriter), finished by close(). png=False leaves the PNGs out; png_mode ("fixed" or "dynamic") is encode_png's
+    mode."""
 
-    def __init__(self, directory, H, W, device, slots=4, png=True, video_fps=None, video_quality=90, video_tag=""):
+    def __init__(self, directory, H, W, device, slots=4, png=True, video_fps=None, video_quality=90, video_tag="",
+                 png_mode="fixed"):
+        _png_mode(png_mode)
         self.dir, self.H, self.W = directory, int(H), int(W)
         os.makedirs(directory, exist_ok=True)
-        self.png, self.quality = bool(png), int(video_quality)
+        self.png, self.quality, self.png_mode = bool(png), int(video_quality), png_mode
         caps = [png_capacity(H, W)] * 2 * self.png + [jpeg_capacity(H, W)] * 2 * (video_fps is not None)
         self.rgb_img = torch.empty(H, W, 3, dtype=torch.uint8, device=device)
         self.depth_img = torch.empty(H, W, 3, dtype=torch.uint8, device=device)
         self.vi_ws = torch.empty(_lib.NGP_VIEW_IMAGES_WORKSPACE, dtype=torch.uint8, device=device)
-        self.png_ws = png_workspace(H, W, device) if self.png else None
+        self.png_ws = png_workspace(H, W, device, png_mode) if self.png else None
         self.jpeg_ws = jpeg_workspace(H, W, device) if video_fps is not None else None
         self.videos = None if video_fps is None else [
             AviWriter(os.path.join(directory, "%s%s.avi" % (name, video_tag)), W, H, video_fps) for name in ("rgb", "depth")]
@@ -323,7 +342,7 @@ class ViewWriter:
         j = 0
         if self.png:
             for img in (self.rgb_img, self.depth_img):
-                encode_png_into(img, s["bufs"][j], s["len"][j:j + 1], self.png_ws)
+                encode_png_into(img, s["bufs"][j], s["len"][j:j + 1], self.png_ws, self.png_mode)
                 j += 1
         if self.videos is not None:
             for img in (self.rgb_img, self.depth_img):

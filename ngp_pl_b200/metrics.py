@@ -225,7 +225,7 @@ def gather_metrics(local, n_views, n_pixels, world_size=1, rank=0, process_group
 
 @torch.no_grad()
 def evaluate(render_fn, poses, directions, images, img_wh, world_size=1, rank=0, process_group=None, exp_step_factor=0.0,
-             lpips_net=None, save_dir=None, video_fps=None, video_quality=90):
+             lpips_net=None, save_dir=None, video_fps=None, video_quality=90, png_mode="fixed"):
     """The reference's validation pass (train.py:193-237): renders this rank's share of the views
     (shard_range, the split bench.py's render_fps uses), runs ngp_image_metrics on each output on the same stream, reads
     the per-view results back once at the end and gathers them over the ranks.
@@ -242,13 +242,17 @@ def evaluate(render_fn, poses, directions, images, img_wh, world_size=1, rank=0,
     i the global view index. render_fn's result must then hold 'depth'. Each view's images and PNGs are enqueued on the
     render stream after its metrics, into a small ring of pinned host slots that one writer thread empties while the GPU
     renders the next view (images.ViewWriter); the stream is not synchronised per view, the call returns once every file
-    is written, and the returned dict is the one without save_dir.
+    is written, and the returned dict is the one without save_dir. png_mode "dynamic" (images.encode_png's mode) writes
+    smaller files of the same arrays; "fixed", the default, is the faster stream.
 
     With video_fps as well (RuntimeError without save_dir), the same two images of every view of the shard, in view
     order, are also the frames of the Motion-JPEG videos `rgb.avi` and `depth.avi` in save_dir (the reference's rgb.mp4
     and depth.mp4, made from those PNGs; images.AviWriter), JPEG-encoded at video_quality on the render stream after the
     PNG encodes. With world_size > 1 each rank writes its shard as `rgb.rank{r}.avi` / `depth.rank{r}.avi`."""
     from . import synth
+    from .images import PNG_MODES
+    if png_mode not in PNG_MODES:
+        raise ValueError("ngp_pl_b200.metrics.evaluate: png_mode must be one of %s, got %r" % (sorted(PNG_MODES), png_mode))
     if isinstance(render_fn, torch.nn.Module):
         from .models.rendering import render
         model = render_fn
@@ -269,7 +273,7 @@ def evaluate(render_fn, poses, directions, images, img_wh, world_size=1, rank=0,
     if save_dir is not None:
         from .images import ViewWriter
         writer = ViewWriter(save_dir, H, W, dev, video_fps=video_fps, video_quality=video_quality,
-                            video_tag=".rank%d" % rank if world_size > 1 else "")
+                            video_tag=".rank%d" % rank if world_size > 1 else "", png_mode=png_mode)
     try:
         for i in range(lo, hi):
             o, d = synth.get_rays(directions, poses[i])
