@@ -99,7 +99,9 @@ int ngp_composite_test_fw(const float* sigmas, const float* rgbs, const float* d
                           const float* hits_t, int64_t* alive_indices, float T_threshold, const int* N_eff_samples,
                           int n_alive, int N_samples, float* opacity, float* depth, float* rgb, void* stream);
 
-/* vren.distortion_loss_fw / _bw (binding.cpp:197-231, losses.cu:10-174). */
+/* vren.distortion_loss_fw / _bw (binding.cpp:197-231, losses.cu:10-174). n_samples is the extent of the per-sample
+ * arrays (ws, deltas, ts, the scans, dL_dws): each ray's segment [start, start + count) is clipped to it, and a ray
+ * clipped to nothing gets loss 0 and no per-sample writes. */
 int ngp_distortion_loss_fw(const float* ws, const float* deltas, const float* ts, const int64_t* rays_a, int n_rays,
                            int64_t n_samples, float* loss, float* ws_inclusive_scan, float* wts_inclusive_scan,
                            void* stream);

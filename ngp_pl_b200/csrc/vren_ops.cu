@@ -591,16 +591,22 @@ extern "C" int ngp_composite_test_fw(const float* sigmas, const float* rgbs, con
 // distortion_loss_fw / distortion_loss_bw  (reference binding.cpp:197-231 -> losses.cu:10-174)
 // One warp per ray; the four thrust scans + elementwise torch ops + reduce of the reference become
 // one pass.
+// Every ray's segment is clipped to the n_samples entries the per-sample arrays hold (the Trainer's capacity may be smaller
+// than what its batch marched, as in train.cu): a ray clipped to nothing gets loss 0 and no per-sample writes.
 // ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ int distortion_extent(int64_t start, int64_t n, int64_t n_samples) {
+    return (int)max((int64_t)0, min(n, n_samples - start));
+}
+
 __global__ void k_distortion_fw(const float* __restrict__ ws, const float* __restrict__ deltas, const float* __restrict__ ts,
-                                const int64_t* __restrict__ rays_a, int n_rays, float* __restrict__ loss,
-                                float* __restrict__ ws_inc, float* __restrict__ wts_inc) {
+                                const int64_t* __restrict__ rays_a, int n_rays, int64_t n_samples,
+                                float* __restrict__ loss, float* __restrict__ ws_inc, float* __restrict__ wts_inc) {
     const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (w >= n_rays) return;
     const int64_t ray = rays_a[3 * w];
     const int64_t start = rays_a[3 * w + 1];
-    const int n = (int)rays_a[3 * w + 2];
+    const int n = distortion_extent(start, rays_a[3 * w + 2], n_samples);
     float cw = 0.f, cwt = 0.f, acc = 0.f;
     for (int base = 0; base < n; base += 32) {
         const int i = base + lane;
@@ -625,11 +631,10 @@ __global__ void k_distortion_fw(const float* __restrict__ ws, const float* __res
 extern "C" int ngp_distortion_loss_fw(const float* ws, const float* deltas, const float* ts, const int64_t* rays_a,
                                       int n_rays, int64_t n_samples, float* loss, float* ws_inclusive_scan,
                                       float* wts_inclusive_scan, void* stream) {
-    (void)n_samples;
-    if (n_rays < 0) return NGP_EINVAL;
+    if (n_rays < 0 || n_samples < 0) return NGP_EINVAL;
     if (n_rays == 0) return 0;
     k_distortion_fw<<<ngp_div_up((int64_t)n_rays * 32, 128), 128, 0, (cudaStream_t)stream>>>(
-        ws, deltas, ts, rays_a, n_rays, loss, ws_inclusive_scan, wts_inclusive_scan);
+        ws, deltas, ts, rays_a, n_rays, n_samples, loss, ws_inclusive_scan, wts_inclusive_scan);
     NGP_CHECK_LAUNCH();
     return 0;
 }
@@ -637,13 +642,14 @@ extern "C" int ngp_distortion_loss_fw(const float* ws, const float* deltas, cons
 __global__ void k_distortion_bw(const float* __restrict__ dL_dloss, const float* __restrict__ ws_inc,
                                 const float* __restrict__ wts_inc, const float* __restrict__ ws,
                                 const float* __restrict__ deltas, const float* __restrict__ ts,
-                                const int64_t* __restrict__ rays_a, int n_rays, float* __restrict__ dL_dws) {
+                                const int64_t* __restrict__ rays_a, int n_rays, int64_t n_samples,
+                                float* __restrict__ dL_dws) {
     const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (w >= n_rays) return;
     const int64_t ray = rays_a[3 * w];
     const int64_t start = rays_a[3 * w + 1];
-    const int n = (int)rays_a[3 * w + 2];
+    const int n = distortion_extent(start, rays_a[3 * w + 2], n_samples);
     if (n <= 0) return;
     const float g = dL_dloss[ray];
     const float ws_sum = ws_inc[start + n - 1];
@@ -660,11 +666,10 @@ __global__ void k_distortion_bw(const float* __restrict__ dL_dloss, const float*
 extern "C" int ngp_distortion_loss_bw(const float* dL_dloss, const float* ws_inclusive_scan, const float* wts_inclusive_scan,
                                       const float* ws, const float* deltas, const float* ts, const int64_t* rays_a,
                                       int n_rays, int64_t n_samples, float* dL_dws, void* stream) {
-    (void)n_samples;
-    if (n_rays < 0) return NGP_EINVAL;
+    if (n_rays < 0 || n_samples < 0) return NGP_EINVAL;
     if (n_rays == 0) return 0;
     k_distortion_bw<<<ngp_div_up((int64_t)n_rays * 32, 128), 128, 0, (cudaStream_t)stream>>>(
-        dL_dloss, ws_inclusive_scan, wts_inclusive_scan, ws, deltas, ts, rays_a, n_rays, dL_dws);
+        dL_dloss, ws_inclusive_scan, wts_inclusive_scan, ws, deltas, ts, rays_a, n_rays, n_samples, dL_dws);
     NGP_CHECK_LAUNCH();
     return 0;
 }

@@ -94,6 +94,61 @@ def composite_case(seed=3, n_rays=96, max_n=300):
     return dict(sigmas=sig, rgbs=rgbs, deltas=deltas, ts=ts, rays_a=rays_a, T_thr=np.float32(1e-4), **g)
 
 
+DISTORTION_LENGTHS = (0, 1, 2, 31, 32, 33, 63, 64, 65, 1023, 1024, 3000)
+
+
+def distortion_case(seed=0, profile="lego", lengths=DISTORTION_LENGTHS, repeat=2, n_long=3, n_random=37):
+    """ragged weights for the distortion loss: every length `repeat` times (3000: n_long times) plus n_random random
+    ones, an odd number of rays in all; the segments lie in scrambled order with gaps between them and rays_a[:, 0] is
+    a permutation of the rows. Weights are those of a compositing pass (a_i T_{i-1}, exact zeros once T <= 1e-4), with
+    an all-zero ray, a ray cut to zeros at a chosen index and a sample within 2^-20 of 1.
+    profile 'lego': t from 0.5 to 1 on, constant step sqrt(3)/1024;
+            'exp16': a scale-16 scene's exponential step, dt = clamp(t / 256, sqrt(3)/1024, 16 * 2 sqrt(3)/128)."""
+    assert profile in ("lego", "exp16")
+    rng = np.random.RandomState(seed)
+    counts = [n for n in lengths for _ in range(n_long if n >= 3000 else repeat)]
+    counts = np.array(counts + list(rng.randint(0, 200, n_random)), np.int64)
+    if len(counts) % 2 == 0:
+        counts = np.append(counts, 5)
+    R = len(counts)
+    gaps = rng.randint(1, 6, R)
+    start = np.zeros(R, np.int64)
+    at = 0
+    for r in rng.permutation(R):  # segments in scrambled order, gaps between them
+        at += gaps[r]
+        start[r] = at
+        at += counts[r]
+    n_buf = at + 7
+    ws, ts, deltas = np.zeros(n_buf, np.float32), np.zeros(n_buf, np.float32), np.zeros(n_buf, np.float32)
+    dmin, dmax = np.float32(1.7320508 / 1024), np.float32(16 * 2 * 1.7320508 / 128)
+    for r in range(R):
+        n, s = int(counts[r]), int(start[r])
+        if profile == "lego":
+            dt = np.full(n, dmin, np.float32)
+            t = (np.float32(0.5 + 0.5 * rng.rand()) + np.arange(n, dtype=np.float32) * dmin).astype(np.float32)
+        else:
+            t, dt = np.zeros(n, np.float32), np.zeros(n, np.float32)
+            tc = np.float32(rng.uniform(0.05, 1.0))
+            for k in range(n):
+                dt[k] = np.clip(tc / np.float32(256), dmin, dmax)
+                t[k] = tc
+                tc = np.float32(tc + dt[k])
+        x = np.exp(rng.normal(np.log(10 ** rng.uniform(-3.5, 0)), 1.5, n))
+        a = -np.expm1(-x)
+        T = np.concatenate([[1.0], np.cumprod(1 - a)[:-1]])
+        w = np.where(T > 1e-4, a * T, 0.0).astype(np.float32)
+        ws[s:s + n], ts[s:s + n], deltas[s:s + n] = w, t, dt
+    by_len = {int(n): r for r, n in enumerate(counts)}
+    zero, cut, peak = by_len[64], by_len[1024], by_len[33]
+    ws[start[zero]:start[zero] + 64] = 0
+    ws[start[cut] + 700:start[cut] + 1024] = 0
+    ws[start[peak]:start[peak] + 33] = np.float32(1e-3)
+    ws[start[peak] + 5] = np.float32(1 - 2 ** -20)
+    ws[start[peak] + 6:start[peak] + 33] = 0
+    rays_a = np.stack([rng.permutation(R), start, counts], 1).astype(np.int64)
+    return dict(ws=ws, ts=ts, deltas=deltas, rays_a=rays_a, special=dict(zero=zero, cut=cut, peak=peak))
+
+
 def composite_test_case():
     """one round of the test-time compositor: 150 of 200 rays alive, up to 8 samples each, running ray state"""
     rng = np.random.RandomState(4)

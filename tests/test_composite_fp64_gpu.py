@@ -11,7 +11,8 @@ termination the bound cannot decide is reported and left out; at most 1 % of a b
 Batches: random-initialised Lego and mip360 models, a briefly trained Lego, a controlled density (constant sigma, so that
 terminations land at chosen lanes of chosen trips) over rays of every length 0..579, a random background, lambda_opacity
 1e-3 and 1, and ray counts that leave spare warps in the last block. The separate-kernel path also gets seeded non-zero
-dL/ddepth and dL/dws, which the Trainer never passes.
+dL/ddepth, which the Trainer never passes, and dL/dws, which the Trainer passes only with lambda_distortion > 0 (the
+distortion kernel's output; test_distortion_fp64_gpu.py checks that path with the kernel's own dL/dws).
 """
 import ctypes as C
 import math
