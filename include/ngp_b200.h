@@ -457,6 +457,38 @@ int ngp_render_infer_frame(const NgpNet* net, const NgpInferCfg* cfg, const floa
                            const uint8_t* density_bitfield, float* opacity, float* depth, float* rgb, int64_t* total_samples,
                            void* workspace, size_t workspace_bytes, void* stream);
 
+/* One frame of the interactive viewer (the reference's show_gui.py render_cam: get_rays, render(test_time=True),
+ * depth2img) as ONE cached CUDA graph, from camera pose to JPEG file:
+ *   1. a memcpy node copies the 3x4 camera-to-world pose (12 floats, row-major [R | t]) from `pose`, which must be
+ *      pinned host memory, into the workspace -- every launch reads the buffer's contents at that moment, so moving the
+ *      camera never rebuilds the graph;
+ *   2. rays_d = directions @ R^T, rays_o = t for every pixel (directions (H*W, 3) device), with ngp_gen_rays' arithmetic:
+ *      rays_o / rays_d (H*W, 3) are bitwise ngp_gen_rays with img_idx = 0, pix_idx = 0 .. H*W-1 on that pose;
+ *   3. the wavefront of ngp_render_infer_frame on those rays (opacity, depth, rgb as it writes them);
+ *   4. ngp_view_images of the chosen output only (mode 0: rgb_img of rgb, 1: depth_img of depth), then ngp_jpeg_encode
+ *      of that image at view->quality into jpeg.
+ * stats (int64[2]): [0] the JPEG's length, [1] total_samples. jpeg and stats may be device memory or mapped pinned host
+ * memory (as for ngp_jpeg_encode), so only the file's bytes cross PCIe; nothing in the call synchronises the stream.
+ * Graphs are cached as ngp_render_infer_frame's are (up to 8, per device, every pointer argument, *net, *cfg and *view):
+ * the two modes are two entries, and toggling between them rebuilds nothing once both exist. Not thread-safe.
+ * workspace: ngp_render_view_workspace(cfg, view) bytes, 256-B aligned -- ngp_render_infer_workspace's, then the pose,
+ * the ngp_view_images workspace, the (H, W, 3) display image and the ngp_jpeg_workspace(H, W) -- or 0 when
+ * H * W != cfg->n_rays or ngp_jpeg_workspace(H, W) is 0. NGP_EINVAL for H * W != n_rays, an unknown mode, a quality
+ * outside 1..100, jpeg_capacity < ngp_jpeg_capacity(H, W), a NULL pointer, a pose that is not pinned host memory, another
+ * pointer the device cannot reach, stats not 8-B aligned, a short or misaligned workspace, and everything
+ * ngp_render_infer_frame refuses. A cudaError_t if the driver cannot build conditional graph nodes; there is no other
+ * path. */
+typedef struct {
+    int32_t mode;    /* 0 = rgb_img, 1 = depth_img (ngp_view_images' two outputs) */
+    int32_t quality; /* JPEG quality 1..100 */
+    int32_t H, W;    /* H * W == cfg->n_rays */
+} NgpViewCfg;
+size_t ngp_render_view_workspace(const NgpInferCfg* cfg, const NgpViewCfg* view);
+int ngp_render_view_frame(const NgpNet* net, const NgpInferCfg* cfg, const NgpViewCfg* view, const float* directions,
+                          const float* pose, const uint8_t* density_bitfield, float* rays_o, float* rays_d, float* opacity,
+                          float* depth, float* rgb, uint8_t* jpeg, size_t jpeg_capacity, int64_t* stats,
+                          void* workspace, size_t workspace_bytes, void* stream);
+
 /* ----------------------------------------------------------------------------------------------
  * Validation metrics of one rendered view (reference train.py:193-237): the per-image PSNR of torchmetrics'
  * PeakSignalNoiseRatio(data_range=1) / metrics.py:14-15 and SSIM of StructuralSimilarityIndexMeasure(data_range=1)

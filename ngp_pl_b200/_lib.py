@@ -103,6 +103,16 @@ class NgpInferCfg(C.Structure):
     ]
 
 
+class NgpViewCfg(C.Structure):
+    """Mirror of NgpViewCfg in include/ngp_b200.h."""
+    _fields_ = [
+        ("mode", C.c_int32),
+        ("quality", C.c_int32),
+        ("H", C.c_int32),
+        ("W", C.c_int32),
+    ]
+
+
 class NgpTrainBuffers(C.Structure):
     """Mirror of NgpTrainBuffers in include/ngp_b200.h."""
     _fields_ = [(n, C.c_void_p) for n in (
@@ -171,6 +181,9 @@ SIGNATURES = {
     "ngp_render_infer": (_i, [C.POINTER(NgpNet), C.POINTER(NgpInferCfg), _P, _P, _P, _P, _P, _P, _P, _i, _i, _i, _P,
                               _P, _sz, _P]),
     "ngp_render_infer_frame": (_i, [C.POINTER(NgpNet), C.POINTER(NgpInferCfg), _P, _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
+    "ngp_render_view_workspace": (_sz, [C.POINTER(NgpInferCfg), C.POINTER(NgpViewCfg)]),
+    "ngp_render_view_frame": (_i, [C.POINTER(NgpNet), C.POINTER(NgpInferCfg), C.POINTER(NgpViewCfg)] + [_P] * 9 +
+                              [_sz, _P, _P, _sz, _P]),
     "ngp_update_grid_workspace": (_sz, [_i, _i]),
     "ngp_update_density_grid": (_i, [C.POINTER(NgpNet), _P, _P, _P, _i, _i, _f, _f, _i, _f, C.c_uint32, _P, _sz, _P]),
     "ngp_update_density_grid_pick": (_i, [_P, _i, _i, _f, _f, _i, C.c_uint32, _P, _sz, _P]),

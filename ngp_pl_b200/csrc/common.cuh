@@ -118,6 +118,19 @@ static inline bool ngp_dev_ptr(const void* p, bool host_mapped_ok) {
     return host_mapped_ok && a.type == cudaMemoryTypeHost && a.devicePointer == p;
 }
 
+// One camera ray (reference datasets/ray_utils.py:46-70): rays_d = direction @ R^T, rays_o = t, for the 3x4
+// camera-to-world pose P = [R | t] (row-major). The batch assembly and the viewer's frames share this arithmetic, so their
+// rays are bitwise equal for the same pose and direction.
+__device__ __forceinline__ void pose_ray(const float* __restrict__ P, float dx, float dy, float dz, float* __restrict__ o,
+                                         float* __restrict__ d) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        // d_k = sum_c dir_c * R[k][c]
+        d[k] = fmaf(dz, P[4 * k + 2], fmaf(dy, P[4 * k + 1], dx * P[4 * k]));
+        o[k] = P[4 * k + 3];
+    }
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -313,6 +313,17 @@ extern "C" size_t ngp_render_infer_workspace(int n_rays, int64_t max_round_sampl
     return 6 * nr + 7 * ns + 4096;
 }
 
+// the arguments every wavefront entry point refuses with NGP_EINVAL
+static bool infer_args_ok(const NgpNet* net, const NgpInferCfg* cfg, const float* rays_o, const float* rays_d,
+                          const uint8_t* density_bitfield, const float* opacity, const float* depth, const float* rgb,
+                          const void* workspace, size_t workspace_bytes) {
+    if (!net || !cfg || !rays_o || !rays_d || !density_bitfield || !opacity || !depth || !rgb || !workspace) return false;
+    if (cfg->n_rays < 1 || cfg->cascades < 1 || cfg->grid_size < 1 || cfg->grid_size > 1024 || cfg->max_samples < 1 ||
+        cfg->max_round_samples < cfg->n_rays || cfg->max_round_samples > 0x7fffffffll || cfg->sample_budget < 1)
+        return false;
+    return workspace_bytes >= ngp_render_infer_workspace(cfg->n_rays, cfg->max_round_samples);
+}
+
 // Runs rounds [first_round, first_round + n_rounds) of the wavefront. first_round == 0 also initialises
 // (AABB, accumulators, first alive list); finish != 0 adds the background and writes total_samples.
 // alive_count_out (device int32*, optional) receives the number of rays still alive after the last round
@@ -322,12 +333,9 @@ extern "C" int ngp_render_infer(const NgpNet* net, const NgpInferCfg* cfg, const
                                 const uint8_t* density_bitfield, float* opacity, float* depth, float* rgb,
                                 int64_t* total_samples, int first_round, int n_rounds, int finish, int* alive_count_out,
                                 void* workspace, size_t workspace_bytes, void* stream) {
-    if (!net || !cfg || !rays_o || !rays_d || !density_bitfield || !opacity || !depth || !rgb || !workspace) return NGP_EINVAL;
-    if (cfg->n_rays < 1 || cfg->cascades < 1 || cfg->grid_size < 1 || cfg->grid_size > 1024 || cfg->max_samples < 1 ||
-        cfg->max_round_samples < cfg->n_rays || cfg->max_round_samples > 0x7fffffffll || cfg->sample_budget < 1 ||
+    if (!infer_args_ok(net, cfg, rays_o, rays_d, density_bitfield, opacity, depth, rgb, workspace, workspace_bytes) ||
         first_round < 0 || n_rounds < 0)
         return NGP_EINVAL;
-    if (workspace_bytes < ngp_render_infer_workspace(cfg->n_rays, cfg->max_round_samples)) return NGP_EINVAL;
     cudaStream_t st = (cudaStream_t)stream;
     const int n = cfg->n_rays;
     const InferWs W = infer_ws(cfg, workspace);
@@ -399,17 +407,13 @@ struct InferGraphKey {
     const void *rays_o, *rays_d, *bitfield, *opacity, *depth, *rgb, *total, *workspace;
     int device;
 };
-struct InferGraphEntry {
-    InferGraphKey key;
-    cudaGraphExec_t exec;
-    cudaGraph_t graph;
-    bool used;
-};
-#define INFER_GRAPH_CACHE 8
-static InferGraphEntry g_infer_graphs[INFER_GRAPH_CACHE];
-static unsigned g_infer_graph_clock = 0;
 
-static int build_infer_graph(const InferGraphKey& k, InferGraphEntry* e) {
+// Builds the frame graph of k: [head(cs)] clear + init -> WHILE { two rounds } -> finish [tail(cs)]. head and tail capture
+// the caller's own nodes (int head(cudaStream_t), 0 or an error) into the graph before the first and after the last
+// node of the wavefront.
+template <typename Head, typename Tail>
+static int build_wavefront_graph(const InferGraphKey& k, Head head, Tail tail, cudaGraph_t* graph_out,
+                                 cudaGraphExec_t* exec_out) {
     const NgpNet* net = &k.net;
     const NgpInferCfg* cfg = &k.cfg;
     const float* rays_o = (const float*)k.rays_o;
@@ -426,20 +430,22 @@ static int build_infer_graph(const InferGraphKey& k, InferGraphEntry* e) {
     int rc = 0;
     do {
         if ((rc = (int)cudaGraphCreate(&g, 0))) break;
-        // ---- head: clear the counters, AABB + first alive list ----
+        // ---- head: the caller's nodes, clear the counters, AABB + first alive list ----
         if ((rc = (int)cudaStreamBeginCaptureToGraph(cs, g, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal))) break;
+        rc = head(cs);
         cudaMemsetAsync(W.counters, 0, 4096, cs);
         k_infer_init<<<ngp_div_up(n, 256), 256, 0, cs>>>(*cfg, rays_o, rays_d, W.t_cur, W.t_end, opacity, depth, rgb, W.alive[0],
                                                           W.alive_cnt, W.alive_cnt + 1, W.state, W.total);
         cudaStreamCaptureStatus status;
         const cudaGraphNode_t* deps = nullptr;
         size_t n_deps = 0;
-        if ((rc = (int)cudaStreamGetCaptureInfo(cs, &status, nullptr, nullptr, &deps, &n_deps))) break;
+        int rc2 = (int)cudaStreamGetCaptureInfo(cs, &status, nullptr, nullptr, &deps, &n_deps);
         cudaGraphNode_t head_tail[8];
-        if (n_deps > 8) { rc = NGP_EINVAL; break; }
-        for (size_t i = 0; i < n_deps; ++i) head_tail[i] = deps[i];
+        if (!rc2 && n_deps > 8) rc2 = NGP_EINVAL;
+        for (size_t i = 0; !rc2 && i < n_deps; ++i) head_tail[i] = deps[i];
         cudaGraph_t tmp = nullptr;
-        if ((rc = (int)cudaStreamEndCapture(cs, &tmp))) break;
+        int rc3 = (int)cudaStreamEndCapture(cs, &tmp);
+        if (rc || (rc = rc2) || (rc = rc3)) break;
         // ---- the WHILE node ----
         cudaGraphConditionalHandle handle;
         if ((rc = (int)cudaGraphConditionalHandleCreate(&handle, g, 1, cudaGraphCondAssignDefault))) break;
@@ -454,19 +460,18 @@ static int build_infer_graph(const InferGraphKey& k, InferGraphEntry* e) {
         if ((rc = (int)cudaStreamBeginCaptureToGraph(cs, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal))) break;
         for (int half = 0; half < 2 && !rc; ++half)  // the second round's compositing sets the loop condition
             rc = infer_round(net, cfg, W, rays_o, rays_d, bitfield, opacity, depth, rgb, half, cs, handle, half);
-        int rc2 = (int)cudaStreamEndCapture(cs, &tmp);
-        if (rc) break;
-        if ((rc = rc2)) break;
-        // ---- tail: background + total ----
+        rc2 = (int)cudaStreamEndCapture(cs, &tmp);
+        if (rc || (rc = rc2)) break;
+        // ---- tail: background + total, the caller's nodes ----
         if ((rc = (int)cudaStreamBeginCaptureToGraph(cs, g, &loop, nullptr, 1, cudaStreamCaptureModeThreadLocal))) break;
         k_infer_finish<<<ngp_div_up(n, 256), 256, 0, cs>>>(*cfg, opacity, rgb, W.state, W.total, (int64_t*)k.total);
-        if ((rc = (int)cudaStreamEndCapture(cs, &tmp))) break;
+        rc = tail(cs);
+        rc2 = (int)cudaStreamEndCapture(cs, &tmp);
+        if (rc || (rc = rc2)) break;
         cudaGraphExec_t exec = nullptr;
         if ((rc = (int)cudaGraphInstantiate(&exec, g, 0))) break;
-        e->exec = exec;
-        e->graph = g;
-        e->key = k;
-        e->used = true;
+        *exec_out = exec;
+        *graph_out = g;
         g = nullptr;
     } while (0);
     if (rc) {
@@ -483,39 +488,177 @@ static int build_infer_graph(const InferGraphKey& k, InferGraphEntry* e) {
     return rc;
 }
 
-extern "C" int ngp_render_infer_frame(const NgpNet* net, const NgpInferCfg* cfg, const float* rays_o, const float* rays_d,
-                                      const uint8_t* density_bitfield, float* opacity, float* depth, float* rgb,
-                                      int64_t* total_samples, void* workspace, size_t workspace_bytes, void* stream) {
-    if (!net || !cfg || !rays_o || !rays_d || !density_bitfield || !opacity || !depth || !rgb || !workspace) return NGP_EINVAL;
-    if (cfg->n_rays < 1 || cfg->cascades < 1 || cfg->grid_size < 1 || cfg->grid_size > 1024 || cfg->max_samples < 1 ||
-        cfg->max_round_samples < cfg->n_rays || cfg->max_round_samples > 0x7fffffffll || cfg->sample_budget < 1)
-        return NGP_EINVAL;
-    if (workspace_bytes < ngp_render_infer_workspace(cfg->n_rays, cfg->max_round_samples)) return NGP_EINVAL;
-    InferGraphKey k;
-    memset(&k, 0, sizeof(k));
-    k.net = *net;
-    k.cfg = *cfg;
-    k.rays_o = rays_o; k.rays_d = rays_d; k.bitfield = density_bitfield; k.opacity = opacity; k.depth = depth; k.rgb = rgb;
-    k.total = total_samples; k.workspace = workspace;
-    NGP_CUDA(cudaGetDevice(&k.device));
-    InferGraphEntry* hit = nullptr;
-    InferGraphEntry* victim = &g_infer_graphs[g_infer_graph_clock % INFER_GRAPH_CACHE];
-    for (int i = 0; i < INFER_GRAPH_CACHE; ++i) {
-        InferGraphEntry* e = &g_infer_graphs[i];
-        if (e->used && memcmp(&e->key, &k, sizeof(k)) == 0) { hit = e; break; }
-        if (!e->used) victim = e;
-    }
-    if (!hit) {
+// Instantiated graphs keyed by the bytes of Key (zero-filled before its fields are set): up to INFER_GRAPH_CACHE
+// entries, an empty slot or the oldest entry rebuilt on a miss. Not thread-safe.
+#define INFER_GRAPH_CACHE 8
+template <typename Key>
+struct GraphCache {
+    struct Entry {
+        Key key;
+        cudaGraphExec_t exec;
+        cudaGraph_t graph;
+        bool used;
+    };
+    Entry e[INFER_GRAPH_CACHE];
+    unsigned tick;
+    // the executable graph of k; on a miss build(k, &graph, &exec) makes it
+    template <typename Build>
+    int get(const Key& k, Build build, cudaGraphExec_t* out) {
+        Entry* victim = &e[tick % INFER_GRAPH_CACHE];
+        for (int i = 0; i < INFER_GRAPH_CACHE; ++i) {
+            if (e[i].used && memcmp(&e[i].key, &k, sizeof(k)) == 0) {
+                *out = e[i].exec;
+                return 0;
+            }
+            if (!e[i].used) victim = &e[i];
+        }
         if (victim->used) {
             cudaGraphExecDestroy(victim->exec);
             cudaGraphDestroy(victim->graph);
             victim->used = false;
         }
-        int rc = build_infer_graph(k, victim);
+        const int rc = build(k, &victim->graph, &victim->exec);
         if (rc) return rc;
-        ++g_infer_graph_clock;
-        hit = victim;
+        victim->key = k;
+        victim->used = true;
+        ++tick;
+        *out = victim->exec;
+        return 0;
     }
-    NGP_CUDA(cudaGraphLaunch(hit->exec, (cudaStream_t)stream));
+};
+static GraphCache<InferGraphKey> g_infer_graphs;
+
+static void infer_key(InferGraphKey* k, const NgpNet* net, const NgpInferCfg* cfg, const float* rays_o, const float* rays_d,
+                      const uint8_t* density_bitfield, float* opacity, float* depth, float* rgb, int64_t* total_samples,
+                      void* workspace) {
+    k->net = *net;
+    k->cfg = *cfg;
+    k->rays_o = rays_o; k->rays_d = rays_d; k->bitfield = density_bitfield; k->opacity = opacity; k->depth = depth;
+    k->rgb = rgb; k->total = total_samples; k->workspace = workspace;
+}
+
+static int no_nodes(cudaStream_t) { return 0; }
+
+extern "C" int ngp_render_infer_frame(const NgpNet* net, const NgpInferCfg* cfg, const float* rays_o, const float* rays_d,
+                                      const uint8_t* density_bitfield, float* opacity, float* depth, float* rgb,
+                                      int64_t* total_samples, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!infer_args_ok(net, cfg, rays_o, rays_d, density_bitfield, opacity, depth, rgb, workspace, workspace_bytes))
+        return NGP_EINVAL;
+    InferGraphKey k;
+    memset(&k, 0, sizeof(k));
+    infer_key(&k, net, cfg, rays_o, rays_d, density_bitfield, opacity, depth, rgb, total_samples, workspace);
+    NGP_CUDA(cudaGetDevice(&k.device));
+    cudaGraphExec_t exec;
+    const int rc = g_infer_graphs.get(k, [](const InferGraphKey& key, cudaGraph_t* g, cudaGraphExec_t* x) {
+        return build_wavefront_graph(key, no_nodes, no_nodes, g, x);
+    }, &exec);
+    if (rc) return rc;
+    NGP_CUDA(cudaGraphLaunch(exec, (cudaStream_t)stream));
+    return 0;
+}
+
+// -------------------------------------------------------------------------------------------------
+// The viewer's frame (the reference's show_gui.py render_cam: get_rays, render(test_time=True), depth2img) as ONE graph:
+// pose memcpy -> rays -> the wavefront above -> the display image -> its JPEG. Moving the camera only changes the pinned
+// pose buffer the memcpy node reads at launch, so a frame is one graph launch whatever the pose.
+// -------------------------------------------------------------------------------------------------
+__global__ void k_view_rays(const float* __restrict__ pose, const float* __restrict__ directions, int n,
+                            float* __restrict__ rays_o, float* __restrict__ rays_d) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    pose_ray(pose, directions[3 * i], directions[3 * i + 1], directions[3 * i + 2], rays_o + 3 * i, rays_d + 3 * i);
+}
+
+// the frame's workspace after the wavefront's: pose (48 B) | ngp_view_images workspace | display image | JPEG workspace
+struct ViewWs {
+    size_t pose, vi, img, jpeg, total;
+};
+static bool view_ws(const NgpInferCfg* cfg, const NgpViewCfg* view, ViewWs* y) {
+    if (cfg->n_rays < 1 || cfg->max_round_samples < 1 || view->H < 1 || view->W < 1 ||
+        (int64_t)view->H * view->W != cfg->n_rays)
+        return false;
+    const size_t jpeg_ws = ngp_jpeg_workspace(view->H, view->W);
+    if (!jpeg_ws) return false;
+    auto align = [](size_t v) { return (v + 255) & ~(size_t)255; };
+    y->pose = align(ngp_render_infer_workspace(cfg->n_rays, cfg->max_round_samples));
+    y->vi = y->pose + 256;
+    y->img = y->vi + align(NGP_VIEW_IMAGES_WORKSPACE);
+    y->jpeg = y->img + align((size_t)cfg->n_rays * 3);
+    y->total = y->jpeg + jpeg_ws;
+    return true;
+}
+
+extern "C" size_t ngp_render_view_workspace(const NgpInferCfg* cfg, const NgpViewCfg* view) {
+    ViewWs y;
+    return cfg && view && view_ws(cfg, view, &y) ? y.total : 0;
+}
+
+struct ViewGraphKey {
+    InferGraphKey infer;
+    NgpViewCfg view;
+    const void *directions, *pose, *jpeg;
+    size_t jpeg_capacity;
+};
+static GraphCache<ViewGraphKey> g_view_graphs;
+
+static int build_view_graph(const ViewGraphKey& k, cudaGraph_t* graph_out, cudaGraphExec_t* exec_out) {
+    ViewWs y;
+    view_ws(&k.infer.cfg, &k.view, &y);
+    uint8_t* ws = (uint8_t*)k.infer.workspace;
+    float* pose_dev = (float*)(ws + y.pose);
+    uint8_t* img = ws + y.img;
+    const NgpViewCfg v = k.view;
+    const int n = k.infer.cfg.n_rays;
+    auto head = [&](cudaStream_t cs) -> int {
+        NGP_CUDA(cudaMemcpyAsync(pose_dev, k.pose, 12 * sizeof(float), cudaMemcpyHostToDevice, cs));
+        k_view_rays<<<ngp_div_up(n, 256), 256, 0, cs>>>(pose_dev, (const float*)k.directions, n, (float*)k.infer.rays_o,
+                                                         (float*)k.infer.rays_d);
+        NGP_CHECK_LAUNCH();
+        return 0;
+    };
+    auto tail = [&](cudaStream_t cs) -> int {
+        const int rc = v.mode == 0 ? ngp_view_images((const float*)k.infer.rgb, nullptr, v.H, v.W, img, nullptr, nullptr, 0, cs)
+                                   : ngp_view_images(nullptr, (const float*)k.infer.depth, v.H, v.W, nullptr, img, ws + y.vi,
+                                                     NGP_VIEW_IMAGES_WORKSPACE, cs);
+        if (rc) return rc;
+        return ngp_jpeg_encode(img, v.H, v.W, v.quality, (uint8_t*)k.jpeg, k.jpeg_capacity, (int64_t*)k.infer.total - 1,
+                               ws + y.jpeg, y.total - y.jpeg, cs);
+    };
+    return build_wavefront_graph(k.infer, head, tail, graph_out, exec_out);
+}
+
+extern "C" int ngp_render_view_frame(const NgpNet* net, const NgpInferCfg* cfg, const NgpViewCfg* view,
+                                     const float* directions, const float* pose, const uint8_t* density_bitfield,
+                                     float* rays_o, float* rays_d, float* opacity, float* depth, float* rgb, uint8_t* jpeg,
+                                     size_t jpeg_capacity, int64_t* stats, void* workspace, size_t workspace_bytes,
+                                     void* stream) {
+    if (!infer_args_ok(net, cfg, rays_o, rays_d, density_bitfield, opacity, depth, rgb, workspace, workspace_bytes))
+        return NGP_EINVAL;
+    ViewWs y;
+    if (!view || !view_ws(cfg, view, &y) || (view->mode != 0 && view->mode != 1) || view->quality < 1 || view->quality > 100)
+        return NGP_EINVAL;
+    if (workspace_bytes < y.total || ((uintptr_t)workspace & 255) || jpeg_capacity < ngp_jpeg_capacity(view->H, view->W) ||
+        ((uintptr_t)stats & 7))
+        return NGP_EINVAL;
+    // everything the graph reads or writes must be reachable from the device; the pose is copied from pinned host memory
+    cudaPointerAttributes pa;
+    if (!pose || cudaPointerGetAttributes(&pa, pose) != cudaSuccess || pa.type != cudaMemoryTypeHost) {
+        cudaGetLastError();
+        return NGP_EINVAL;
+    }
+    if (!ngp_dev_ptr(directions, false) || !ngp_dev_ptr(density_bitfield, false) || !ngp_dev_ptr(rays_o, false) ||
+        !ngp_dev_ptr(rays_d, false) || !ngp_dev_ptr(opacity, false) || !ngp_dev_ptr(depth, false) ||
+        !ngp_dev_ptr(rgb, false) || !ngp_dev_ptr(workspace, false) || !ngp_dev_ptr(jpeg, true) || !ngp_dev_ptr(stats, true))
+        return NGP_EINVAL;
+    ViewGraphKey k;
+    memset(&k, 0, sizeof(k));
+    infer_key(&k.infer, net, cfg, rays_o, rays_d, density_bitfield, opacity, depth, rgb, stats + 1, workspace);
+    NGP_CUDA(cudaGetDevice(&k.infer.device));
+    k.view = *view;
+    k.directions = directions; k.pose = pose; k.jpeg = jpeg; k.jpeg_capacity = jpeg_capacity;
+    cudaGraphExec_t exec;
+    const int rc = g_view_graphs.get(k, build_view_graph, &exec);
+    if (rc) return rc;
+    NGP_CUDA(cudaGraphLaunch(exec, (cudaStream_t)stream));
     return 0;
 }

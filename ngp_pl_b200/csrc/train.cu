@@ -966,13 +966,7 @@ __global__ void k_gen_rays(const int64_t* __restrict__ img_idx, const int64_t* _
     if (i >= n) return;
     const int64_t im = img_idx[i], px = pix_idx[i];
     const float* P = poses + 12 * im;
-    const float dx = directions[3 * px], dy = directions[3 * px + 1], dz = directions[3 * px + 2];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        // rays_d = directions @ R^T  ->  d_k = sum_c dir_c * R[k][c]
-        rays_d[3 * i + k] = fmaf(dz, P[4 * k + 2], fmaf(dy, P[4 * k + 1], dx * P[4 * k]));
-        rays_o[3 * i + k] = P[4 * k + 3];
-    }
+    pose_ray(P, directions[3 * px], directions[3 * px + 1], directions[3 * px + 2], rays_o + 3 * i, rays_d + 3 * i);
     if (images && rgb_gt) {
         const uint8_t* c = images + 3 * (im * n_pix + px);
         rgb_gt[3 * i] = c[0] * (1.0f / 255.0f);
