@@ -433,6 +433,39 @@ typedef struct {
 } NgpInferCfg;
 
 size_t ngp_render_infer_workspace(int n_rays, int64_t max_round_samples); /* workspace of ngp_render_infer */
+
+/* Where the wavefront keeps its per-round state inside that workspace, for callers that inspect it between rounds of
+ * ngp_render_infer. Fills offsets[NGP_INFER_LAYOUT_FIELDS] with the byte offset of each array below (offsets may be
+ * NULL) and returns the workspace size, ngp_render_infer_workspace's value; 0 when n_rays or max_round_samples < 1.
+ *   per ray r (n_rays entries):        T_CUR (float) next parameter to march from; T_END (float) the box exit
+ *                                      (-1 for a miss)
+ *   per alive-list position i:         ALIVE0 / ALIVE1 (int32) the two alive lists, ray ids; round k reads list k & 1
+ *                                      and appends the survivors to the other, in no particular order;
+ *                                      RAY_START / RAY_N (int32) first slot and sample count of alive[i] this round
+ *   per slot (max_round_samples):      RAY_IDX (int32, -1 = unused slot), TS, DELTAS, SIGMAS (float), RGBS (float x 3)
+ *   COUNTERS: int32 alive counts of list 0 and 1 at bytes 0 and 4; int32 state[7] at NGP_INFER_STATE_OFFSET:
+ *     state[0] N_samples of the coming round (0 = loop over)  [1] samples requested so far (the reference's `samples`)
+ *     [2] slots the network evaluates this round  [3] rounds run  [4] samples marched this round
+ *     [5] 1 = warp-per-ray marching (N_samples >= 8), 0 = thread-per-ray  [6] finished-block ticket (0 between rounds);
+ *   and the int64 running total of marched samples at NGP_INFER_TOTAL_OFFSET (total_samples = it + state[4]).
+ * In the thread-per-ray regime the rays' slot ranges are packed into [0, state[2]); in the warp-per-ray regime ray i
+ * owns slots [i * N_samples, (i + 1) * N_samples) and state[2] = N_alive * N_samples. */
+#define NGP_INFER_T_CUR 0
+#define NGP_INFER_T_END 1
+#define NGP_INFER_ALIVE0 2
+#define NGP_INFER_ALIVE1 3
+#define NGP_INFER_RAY_START 4
+#define NGP_INFER_RAY_N 5
+#define NGP_INFER_RAY_IDX 6
+#define NGP_INFER_TS 7
+#define NGP_INFER_DELTAS 8
+#define NGP_INFER_SIGMAS 9
+#define NGP_INFER_RGBS 10
+#define NGP_INFER_COUNTERS 11
+#define NGP_INFER_LAYOUT_FIELDS 12
+#define NGP_INFER_STATE_OFFSET 32 /* bytes into COUNTERS */
+#define NGP_INFER_TOTAL_OFFSET 64 /* bytes into COUNTERS */
+size_t ngp_render_infer_layout(int n_rays, int64_t max_round_samples, int64_t* offsets);
 /* Runs rounds [first_round, first_round+n_rounds) of the wavefront (first_round == 0 initialises; finish != 0
  * adds the background and writes total_samples). Per round every alive ray takes up to the reference's quota
  * N_samples = max(min(n_rays / n_alive, 64), min_samples) (rendering.py:73,80; min_samples = 1 if exp_step_factor == 0

@@ -18,6 +18,11 @@ NGP_MC_SLAB_POINTS = 1 << 20
 NGP_VIEW_IMAGES_WORKSPACE = 4096
 NGP_PNG_FIXED = 0
 NGP_PNG_DYNAMIC = 1
+# ngp_render_infer_layout's fields, in the order of NGP_INFER_T_CUR .. NGP_INFER_COUNTERS
+NGP_INFER_FIELDS = ("t_cur", "t_end", "alive0", "alive1", "ray_start", "ray_n", "ray_idx", "ts", "deltas", "sigmas",
+                    "rgbs", "counters")
+NGP_INFER_STATE_OFFSET = 32
+NGP_INFER_TOTAL_OFFSET = 64
 
 
 class NgpGridMeta(C.Structure):
@@ -178,6 +183,7 @@ SIGNATURES = {
     "ngp_sample_rays_ex": (_i, [_P, _P, _P, _i, _i, _i, _i64, _i, C.c_uint32, C.c_uint32, _P, _P, _P, _P, _P, _P]),
     "ngp_stage_image": (_i, [_P, _i, _i, _i, _i, _i, _i, _P, _P]),
     "ngp_render_infer_workspace": (_sz, [_i, _i64]),
+    "ngp_render_infer_layout": (_sz, [_i, _i64, _P]),
     "ngp_render_infer": (_i, [C.POINTER(NgpNet), C.POINTER(NgpInferCfg), _P, _P, _P, _P, _P, _P, _P, _i, _i, _i, _P,
                               _P, _sz, _P]),
     "ngp_render_infer_frame": (_i, [C.POINTER(NgpNet), C.POINTER(NgpInferCfg), _P, _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
@@ -233,6 +239,15 @@ def check(rc, what):
     if rc != 0:
         raise RuntimeError("ngp_pl_b200.%s failed with code %d%s" % (
             what, rc, " (invalid argument)" if rc == -22 else " (cudaError_t)"))
+
+
+def infer_layout(n_rays, max_round_samples):
+    """byte offsets of the wavefront's workspace arrays, {field: offset}, and the workspace size"""
+    off = (C.c_int64 * len(NGP_INFER_FIELDS))()
+    size = lib().ngp_render_infer_layout(int(n_rays), int(max_round_samples), off)
+    if size == 0:
+        raise ValueError("ngp_render_infer_layout: n_rays and max_round_samples must be >= 1")
+    return dict(zip(NGP_INFER_FIELDS, off)), int(size)
 
 
 def grid_meta(n_levels, log2_hashmap_size, base_resolution, per_level_scale):

@@ -277,26 +277,43 @@ struct InferWs {
     int *counters, *alive_cnt, *state;
     int64_t* total;
 };
+// the counter block: [0],[1] alive counts (ping-pong)  [8..14] state  [16..17] int64 total
+#define INFER_COUNTER_BYTES 4096
+
+extern "C" size_t ngp_render_infer_layout(int n_rays, int64_t max_round_samples, int64_t* offsets) {
+    if (n_rays < 1 || max_round_samples < 1) return 0;
+    const size_t nr = ((size_t)n_rays * 4 + 255) & ~(size_t)255;
+    const size_t ns = ((size_t)max_round_samples * 4 + 255) & ~(size_t)255;
+    // t_cur, t_end, alive[0], alive[1], ray_start, ray_n | ray_idx, ts, deltas, sigmas, rgbs (3 per sample) | counters
+    const size_t bytes[NGP_INFER_LAYOUT_FIELDS] = {nr, nr, nr, nr, nr, nr, ns, ns, ns, ns, 3 * ns, INFER_COUNTER_BYTES};
+    size_t at = 0;
+    for (int f = 0; f < NGP_INFER_LAYOUT_FIELDS; ++f) {
+        if (offsets) offsets[f] = (int64_t)at;
+        at += bytes[f];
+    }
+    return at;
+}
+
 static InferWs infer_ws(const NgpInferCfg* cfg, void* workspace) {
-    const size_t nr = ((size_t)cfg->n_rays * 4 + 255) & ~(size_t)255;
-    const size_t ns = ((size_t)cfg->max_round_samples * 4 + 255) & ~(size_t)255;
+    int64_t off[NGP_INFER_LAYOUT_FIELDS];
+    ngp_render_infer_layout(cfg->n_rays, cfg->max_round_samples, off);
     char* w = (char*)workspace;
     InferWs W;
-    W.t_cur = (float*)w; w += nr;
-    W.t_end = (float*)w; w += nr;
-    W.alive[0] = (int*)w; w += nr;
-    W.alive[1] = (int*)w; w += nr;
-    W.ray_start = (int*)w; w += nr;
-    W.ray_n = (int*)w; w += nr;
-    W.ray_idx = (int*)w; w += ns;
-    W.ts = (float*)w; w += ns;
-    W.deltas = (float*)w; w += ns;
-    W.sigmas = (float*)w; w += ns;
-    W.rgbs = (float*)w; w += 3 * ns;
-    W.counters = (int*)w;  // [0],[1] alive counts (ping-pong)  [8..11] state  [16..17] int64 total
+    W.t_cur = (float*)(w + off[NGP_INFER_T_CUR]);
+    W.t_end = (float*)(w + off[NGP_INFER_T_END]);
+    W.alive[0] = (int*)(w + off[NGP_INFER_ALIVE0]);
+    W.alive[1] = (int*)(w + off[NGP_INFER_ALIVE1]);
+    W.ray_start = (int*)(w + off[NGP_INFER_RAY_START]);
+    W.ray_n = (int*)(w + off[NGP_INFER_RAY_N]);
+    W.ray_idx = (int*)(w + off[NGP_INFER_RAY_IDX]);
+    W.ts = (float*)(w + off[NGP_INFER_TS]);
+    W.deltas = (float*)(w + off[NGP_INFER_DELTAS]);
+    W.sigmas = (float*)(w + off[NGP_INFER_SIGMAS]);
+    W.rgbs = (float*)(w + off[NGP_INFER_RGBS]);
+    W.counters = (int*)(w + off[NGP_INFER_COUNTERS]);
     W.alive_cnt = W.counters;
-    W.state = W.counters + 8;
-    W.total = (int64_t*)(W.counters + 16);
+    W.state = W.counters + NGP_INFER_STATE_OFFSET / 4;
+    W.total = (int64_t*)(W.counters + NGP_INFER_TOTAL_OFFSET / 4);
     return W;
 }
 
@@ -306,11 +323,7 @@ static int infer_round(const NgpNet* net, const NgpInferCfg* cfg, const InferWs&
                        cudaGraphConditionalHandle handle = 0, int set_cond = 0);
 
 extern "C" size_t ngp_render_infer_workspace(int n_rays, int64_t max_round_samples) {
-    if (n_rays < 1 || max_round_samples < 1) return 0;
-    const size_t nr = ((size_t)n_rays * 4 + 255) & ~(size_t)255;
-    const size_t ns = ((size_t)max_round_samples * 4 + 255) & ~(size_t)255;
-    // t_cur, t_end, alive[2], ray_start, ray_n  |  ray_idx, ts, deltas, sigmas, rgbs(3)  |  counters
-    return 6 * nr + 7 * ns + 4096;
+    return ngp_render_infer_layout(n_rays, max_round_samples, nullptr);
 }
 
 // the arguments every wavefront entry point refuses with NGP_EINVAL
@@ -344,7 +357,7 @@ extern "C" int ngp_render_infer(const NgpNet* net, const NgpInferCfg* cfg, const
     int64_t* total = W.total;
 
     if (first_round == 0) {
-        NGP_CUDA(cudaMemsetAsync(W.counters, 0, 4096, st));
+        NGP_CUDA(cudaMemsetAsync(W.counters, 0, INFER_COUNTER_BYTES, st));
         NGP_COUNT_LAUNCHES(1);
         k_infer_init<<<ngp_div_up(n, 256), 256, 0, st>>>(*cfg, rays_o, rays_d, W.t_cur, W.t_end, opacity, depth, rgb, W.alive[0],
                                                           alive_cnt, alive_cnt + 1, W.state, W.total);
@@ -433,7 +446,7 @@ static int build_wavefront_graph(const InferGraphKey& k, Head head, Tail tail, c
         // ---- head: the caller's nodes, clear the counters, AABB + first alive list ----
         if ((rc = (int)cudaStreamBeginCaptureToGraph(cs, g, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal))) break;
         rc = head(cs);
-        cudaMemsetAsync(W.counters, 0, 4096, cs);
+        cudaMemsetAsync(W.counters, 0, INFER_COUNTER_BYTES, cs);
         k_infer_init<<<ngp_div_up(n, 256), 256, 0, cs>>>(*cfg, rays_o, rays_d, W.t_cur, W.t_end, opacity, depth, rgb, W.alive[0],
                                                           W.alive_cnt, W.alive_cnt + 1, W.state, W.total);
         cudaStreamCaptureStatus status;
