@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 8
+#define NGP_ABI_VERSION 9
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -612,6 +612,77 @@ int ngp_marching_cubes_count(const float* volume, const NgpLattice* lat, float i
 int ngp_marching_cubes_emit(const float* volume, const NgpLattice* lat, float iso, float* vertices, float* normals,
                             int64_t* triangles, int64_t max_vertices, int64_t max_triangles, void* workspace,
                             size_t workspace_bytes, void* stream);
+
+/* Sparse mesh extraction: sigma and marching cubes only where the occupancy grid says the field can have a surface.
+ * The lattice (n[a] in [2, NGP_MESH_MAX_N]) is cut into bricks of NGP_MESH_BRICK (B) points per axis: point (i, j, k)
+ * belongs to brick (i/B, j/B, k/B), bricks on the upper border may be partial, there are nb[a] = ceil(n[a]/B) per axis
+ * and brick (bi, bj, bk) has linear index (bi*nb1 + bj)*nb2 + bk. A brick mask holds bit (b & 31) of word b >> 5 for
+ * brick b, ngp_mesh_bricks_bytes(lat) bytes.
+ *
+ * Brick mask (ngp_mesh_brick_mask; numpy restatement: oracle/mesh_bricks.py). From the brick's lower and upper corner
+ * points x0, x1 (per axis: the lattice formula at b*B and at min(b*B + B - 1, n - 1)):
+ *   - near = max_a (0 if the axis interval [x0, x1] holds 0, else min(|x0|, |x1|)), far = max_a max(|x0|, |x1|);
+ *   - mip(v) = min(cascades - 1, max(0, e + 1)) with frexpf(v, &e): the marcher's position rule (march.cuh march_probe)
+ *     without its dt term, i.e. the finest cascade whose box holds a point of max-norm v; mip(0) = min(cascades - 1, 1);
+ *   - the cascades taken are c_lo = (near > 0 ? mip(near) : 0) .. c_hi = max(mip(far), near > 0 ? 0 : mip(0));
+ *   - in cascade c, mb = fminf(scalbnf(1, c - 1), scale), inv = 1/mb (fp32 division), and a coordinate x has cell
+ *     coordinate v = (fma(x, inv, 1) * 0.5) * G (fp32, the marcher's cell formula, monotone in x). A point with v < 0 or
+ *     v > G on some axis lies outside cascade c's box: if the brick's [v(x0), v(x1)] lies wholly outside [0, G] on an
+ *     axis, cascade c contributes nothing (points outside the largest cascade's box find no occupancy: no clamping to
+ *     its border cells). Otherwise the cell range is [(int)clamp(v(x0), 0, G-1) - 1, (int)clamp(v(x1), 0, G-1) + 1]
+ *     clipped to [0, G) -- the brick's cells widened by one on every side;
+ *   - the brick is active iff a bit of density_bitfield (cell c*G^3 + morton(x, y, z)) is set in one of those ranges.
+ * This is a superset of the per-point rule "a cell in the 27-neighbourhood of the point's cell, in the cascade of its
+ * position, is occupied", and exact for a brick that lies in one cascade.
+ *
+ * sigma_masked is sigma (bitwise ngp_density_lattice) at the points of active bricks and 0 at every other point. The
+ * sparse extraction returns exactly ngp_marching_cubes_count / _emit of sigma_masked at `iso`: the same vertices in the
+ * same order, the same triangles and the same normals, bitwise. iso must be > 0 (the 0 fill would count as inside
+ * otherwise); a surface that runs into an inactive brick is closed there. No float atomics: two calls are bitwise equal.
+ *
+ * Three steps, each a host call:
+ *   1. ngp_mesh_sparse_bricks: a brick is *visited* when its (B+1)^3 block (the brick plus a one-point apron on the
+ *      upper side, clipped to the lattice) holds a point of an active brick. Pass 1 walks the visited bricks in linear
+ *      order, NGP_MESH_CHUNK_BRICKS at a time, evaluates sigma_masked on their blocks and keeps the *surface* bricks:
+ *      those with a crossed cell (lower corner in the brick) or a crossed edge (lower end in the brick). Every crossed
+ *      cell and edge lies in a visited brick, since an unvisited block is all 0. Writes {active, visited, surface}
+ *      brick counts to the host int64[3] `counts` (two read-backs, so the call synchronises the stream).
+ *   2. ngp_mesh_sparse_count: evaluates sigma_masked again on the surface bricks' (B+3)^3 blocks (one point of apron
+ *      below, two above: what the normals' central differences reach) and stores them in `surface_ws`, counts the
+ *      vertices and triangles of each row of each brick and scans them in the lattice's linear order (rows of B points
+ *      ordered by (i, j, brick column), which is point order and cell order). Writes {n_vertices, n_triangles} to the
+ *      host int64[2] `counts` (a read-back).
+ *   3. ngp_mesh_sparse_emit: writes the mesh as ngp_marching_cubes_emit does, including its capacity check (a
+ *      read-back; NGP_EINVAL with nothing written when max_vertices or max_triangles is short).
+ * The same lattice, iso, mask, net and workspaces go to every step, nothing else touching the workspaces in between.
+ * Device memory: the mask, `workspace` (fixed: two more brick bitmasks, a word prefix and one chunk of sigma blocks)
+ * and `surface_ws` (grows with the surface bricks, 4 (B+3)^3 + 16 B^2 + 28 bytes each), never with the active bricks.
+ * All return NGP_EINVAL for a NULL pointer (other than normals), a lattice outside the limits, iso <= 0 (or NaN) or a
+ * short workspace; the workspace queries return 0 for a lattice outside the limits. */
+#define NGP_MESH_BRICK 8
+#define NGP_MESH_MAX_N 8192
+#define NGP_MESH_CHUNK_BRICKS (1 << 16)
+size_t ngp_mesh_bricks_bytes(const NgpLattice* lat);
+/* The brick mask of `lat` over an occupancy bitfield (cascades * G^3 bits, G a power of two in [2, 1024], cascades in
+ * [1, 62], scale > 0), one thread per brick, no atomics. */
+int ngp_mesh_brick_mask(const uint8_t* density_bitfield, int cascades, int grid_size, float scale, const NgpLattice* lat,
+                        uint32_t* mask, void* stream);
+/* sigma_masked on the blocks of a list of bricks (linear indices, any order): brick s's block is the (W)^3 points from
+ * b*B - apron on each axis, W = B + 1 + 2 * apron (apron 0 or 1), written to sigma[s*W^3 + (li*W + lj)*W + lk]; 0 at
+ * points outside the lattice and at points of bricks whose bit in `mask` is clear (mask NULL: every brick active). The
+ * points are those of ngp_density_lattice, through the same network kernel, so sigma is bitwise its value there. */
+int ngp_density_bricks(const NgpNet* net, const NgpLattice* lat, const int32_t* bricks, int64_t n_bricks, int apron,
+                       const uint32_t* mask, float* sigma, void* stream);
+size_t ngp_mesh_sparse_workspace(const NgpLattice* lat);
+int ngp_mesh_sparse_bricks(const NgpNet* net, const NgpLattice* lat, float iso, const uint32_t* mask, int64_t* counts,
+                           void* workspace, size_t workspace_bytes, void* stream);
+size_t ngp_mesh_surface_workspace(const NgpLattice* lat, int64_t n_surface);
+int ngp_mesh_sparse_count(const NgpNet* net, const NgpLattice* lat, float iso, const uint32_t* mask, int64_t n_surface,
+                          int64_t* counts, void* workspace, size_t workspace_bytes, void* surface_ws, size_t surface_bytes,
+                          void* stream);
+int ngp_mesh_sparse_emit(const NgpLattice* lat, float iso, int64_t n_surface, float* vertices, float* normals,
+                         int64_t* triangles, int64_t max_vertices, int64_t max_triangles, void* surface_ws,
+                         size_t surface_bytes, void* stream);
 
 /* ----------------------------------------------------------------------------------------------
  * Test-view images of the validation pass (reference train.py:215-221): `{idx:03d}.png` holds (rgb_pred*255).astype(np.uint8)

@@ -9,12 +9,15 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 8  #NGP_ABI_VERSION in include/ngp_b200.h
+ABI_VERSION = 9  #NGP_ABI_VERSION in include/ngp_b200.h
 
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
 NGP_RGB_MLP_PARAMS = 7168
 NGP_MC_SLAB_POINTS = 1 << 20
+NGP_MESH_BRICK = 8
+NGP_MESH_MAX_N = 8192
+NGP_MESH_CHUNK_BRICKS = 1 << 16
 NGP_VIEW_IMAGES_WORKSPACE = 4096
 NGP_PNG_FIXED = 0
 NGP_PNG_DYNAMIC = 1
@@ -203,6 +206,14 @@ SIGNATURES = {
     "ngp_marching_cubes_workspace": (_sz, [C.POINTER(NgpLattice)]),
     "ngp_marching_cubes_count": (_i, [_P, C.POINTER(NgpLattice), _f, _P, _P, _sz, _P]),
     "ngp_marching_cubes_emit": (_i, [_P, C.POINTER(NgpLattice), _f, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
+    "ngp_mesh_bricks_bytes": (_sz, [C.POINTER(NgpLattice)]),
+    "ngp_mesh_brick_mask": (_i, [_P, _i, _i, _f, C.POINTER(NgpLattice), _P, _P]),
+    "ngp_density_bricks": (_i, [C.POINTER(NgpNet), C.POINTER(NgpLattice), _P, _i64, _i, _P, _P, _P]),
+    "ngp_mesh_sparse_workspace": (_sz, [C.POINTER(NgpLattice)]),
+    "ngp_mesh_sparse_bricks": (_i, [C.POINTER(NgpNet), C.POINTER(NgpLattice), _f, _P, _P, _P, _sz, _P]),
+    "ngp_mesh_surface_workspace": (_sz, [C.POINTER(NgpLattice), _i64]),
+    "ngp_mesh_sparse_count": (_i, [C.POINTER(NgpNet), C.POINTER(NgpLattice), _f, _P, _i64, _P, _P, _sz, _P, _sz, _P]),
+    "ngp_mesh_sparse_emit": (_i, [C.POINTER(NgpLattice), _f, _i64, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
     "ngp_view_images": (_i, [_P, _P, _i, _i, _P, _P, _P, _sz, _P]),
     "ngp_png_workspace": (_sz, [_i, _i]),
     "ngp_png_capacity": (_sz, [_i, _i]),

@@ -192,6 +192,11 @@ __device__ __forceinline__ SampleIn load_sample(const NgpSamples& s, int64_t i, 
 // a point of a lattice, generated from its row-major index: x = lo + (float)i * step, an fp32 multiply then an fp32 add,
 // so the points are bitwise those a caller materialises with the same formula
 __device__ __forceinline__ int64_t sample_count(const NgpLattice& lat) { return (int64_t)lat.n[0] * lat.n[1] * lat.n[2]; }
+__device__ __forceinline__ void lattice_point(const NgpLattice& lat, int64_t i, int64_t j, int64_t k, SampleIn& s) {
+    s.x = __fadd_rn(lat.lo[0], __fmul_rn((float)i, lat.step[0]));
+    s.y = __fadd_rn(lat.lo[1], __fmul_rn((float)j, lat.step[1]));
+    s.z = __fadd_rn(lat.lo[2], __fmul_rn((float)k, lat.step[2]));
+}
 __device__ __forceinline__ SampleIn load_sample(const NgpLattice& lat, int64_t row, bool& valid) {
     SampleIn s;
     s.x = s.y = s.z = 0.f;
@@ -200,10 +205,47 @@ __device__ __forceinline__ SampleIn load_sample(const NgpLattice& lat, int64_t r
         const int64_t n1 = lat.n[1], n2 = lat.n[2];
         const int64_t k = row % n2, ij = row / n2;
         const int64_t j = ij % n1, i = ij / n1;
-        s.x = __fadd_rn(lat.lo[0], __fmul_rn((float)i, lat.step[0]));
-        s.y = __fadd_rn(lat.lo[1], __fmul_rn((float)j, lat.step[1]));
-        s.z = __fadd_rn(lat.lo[2], __fmul_rn((float)k, lat.step[2]));
+        lattice_point(lat, i, j, k, s);
     }
+    return s;
+}
+
+// the points of a list of lattice bricks (sparse mesh extraction, csrc/mesh.cu): brick s's block is W^3 points from
+// b*B - apron per axis, row s*W^3 + (li*W + lj)*W + lk. Points outside the lattice or in a brick whose mask bit is clear
+// are not evaluated (the caller has zeroed sigma); the others are lattice points, bitwise.
+struct BrickRows {
+    NgpLattice lat;
+    const int32_t* bricks;
+    const uint32_t* mask;  // NULL: every brick active
+    int64_t n_bricks;
+    int32_t nb1, nb2, apron, width;
+};
+__device__ __forceinline__ int64_t sample_count(const BrickRows& b) {
+    return b.n_bricks * (int64_t)(b.width * b.width * b.width);
+}
+__device__ __forceinline__ SampleIn load_sample(const BrickRows& b, int64_t row, bool& valid) {
+    SampleIn s;
+    s.x = s.y = s.z = 0.f;
+    s.dx = 0.f; s.dy = 0.f; s.dz = 1.f;
+    if (!valid) return s;
+    const int w = b.width, w3 = w * w * w;
+    const int brick = __ldg(b.bricks + row / w3), l = (int)(row % w3);
+    const int bk = brick % b.nb2, bij = brick / b.nb2, bj = bij % b.nb1, bi = bij / b.nb1;
+    const int64_t i = (int64_t)bi * NGP_MESH_BRICK - b.apron + l / (w * w);
+    const int64_t j = (int64_t)bj * NGP_MESH_BRICK - b.apron + (l / w) % w;
+    const int64_t k = (int64_t)bk * NGP_MESH_BRICK - b.apron + l % w;
+    if (i < 0 || j < 0 || k < 0 || i >= b.lat.n[0] || j >= b.lat.n[1] || k >= b.lat.n[2]) {
+        valid = false;
+        return s;
+    }
+    if (b.mask) {
+        const int64_t pb = ((i / NGP_MESH_BRICK) * b.nb1 + j / NGP_MESH_BRICK) * b.nb2 + k / NGP_MESH_BRICK;
+        if (!((__ldg(b.mask + (pb >> 5)) >> (pb & 31)) & 1u)) {
+            valid = false;
+            return s;
+        }
+    }
+    lattice_point(b.lat, i, j, k, s);
     return s;
 }
 
@@ -361,6 +403,31 @@ extern "C" int ngp_density_lattice(const NgpNet* net, const NgpLattice* lat, flo
     const int64_t n = (int64_t)lat->n[0] * lat->n[1] * lat->n[2];
     k_ngp_fwd<NgpLattice><<<fwd_grid(n), FWD_THREADS, 0, (cudaStream_t)stream>>>(*net, *lat, 0, sigma, nullptr, nullptr, nullptr,
                                                                                   nullptr);
+    NGP_CHECK_LAUNCH();
+    return 0;
+}
+
+// sigma_masked on the blocks of a brick list (include/ngp_b200.h): zero the blocks, then evaluate the points that count
+extern "C" int ngp_density_bricks(const NgpNet* net, const NgpLattice* lat, const int32_t* bricks, int64_t n_bricks, int apron,
+                                  const uint32_t* mask, float* sigma, void* stream) {
+    if (!net || !lat || !bricks || !sigma || !net->enc_params_h || n_bricks < 0 || (apron != 0 && apron != 1)) return NGP_EINVAL;
+    if (net->meta.n_levels < 1 || net->meta.n_levels > NGP_MAX_LEVELS) return NGP_EINVAL;
+    for (int a = 0; a < 3; ++a)
+        if (lat->n[a] < 2 || lat->n[a] > NGP_MESH_MAX_N) return NGP_EINVAL;
+    if (n_bricks == 0) return 0;
+    BrickRows b;
+    b.lat = *lat;
+    b.bricks = bricks;
+    b.mask = mask;
+    b.n_bricks = n_bricks;
+    b.nb1 = (lat->n[1] + NGP_MESH_BRICK - 1) / NGP_MESH_BRICK;
+    b.nb2 = (lat->n[2] + NGP_MESH_BRICK - 1) / NGP_MESH_BRICK;
+    b.apron = apron;
+    b.width = NGP_MESH_BRICK + 1 + 2 * apron;
+    const int64_t n = n_bricks * (int64_t)(b.width * b.width * b.width);
+    cudaStream_t st = (cudaStream_t)stream;
+    NGP_CUDA(cudaMemsetAsync(sigma, 0, n * sizeof(float), st));
+    k_ngp_fwd<BrickRows><<<fwd_grid(n), FWD_THREADS, 0, st>>>(*net, b, 0, sigma, nullptr, nullptr, nullptr, nullptr);
     NGP_CHECK_LAUNCH();
     return 0;
 }

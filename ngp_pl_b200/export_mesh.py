@@ -1,0 +1,108 @@
+"""Export the mesh of a trained checkpoint as a binary PLY.
+
+    python -m ngp_pl_b200.export_mesh --ckpt_path ckpts/nsvf/Lego/epoch=29.ckpt [--scale 0.5] [--resolution 1024]
+        [--threshold 20] [--bounds x0 y0 z0 x1 y1 z1] [--colors] [--no_normals] [--dense] [--out mesh.ply]
+
+The checkpoint is the full or the slim one train.py writes; it is loaded into NGP(scale) with train.load_weights. By
+default the mesh is mesh.extract_mesh_sparse's: σ evaluated and marching cubes run only near the cells the model's
+occupancy grid marks, so 2048^3 and 4096^3 lattices fit in memory. --dense gives mesh.extract_mesh's mesh of the whole
+lattice (the notebook's mesh cell): a different mesh, which also has the surfaces the occupancy grid has culled.
+Bad arguments are refused with exit status 2 before torch is imported.
+"""
+import argparse
+import math
+import sys
+import time
+
+
+def get_parser():
+    p = argparse.ArgumentParser(prog="python -m ngp_pl_b200.export_mesh",
+                                description="Write the mesh of a trained Instant-NGP checkpoint as a binary PLY.")
+    p.add_argument("--ckpt_path", type=str, required=True, help="full or slim checkpoint of train.py")
+    p.add_argument("--scale", type=float, default=0.5, help="scene scale the model was trained with")
+    p.add_argument("--resolution", type=int, default=1024, help="lattice points per axis, 2..8192")
+    p.add_argument("--threshold", type=float, default=20.0, help="σ level of the surface, > 0")
+    p.add_argument("--bounds", type=float, nargs=6, default=None, metavar=("X0", "Y0", "Z0", "X1", "Y1", "Z1"),
+                   help="lattice box (default: the model's box [-scale, scale]^3)")
+    p.add_argument("--colors", action="store_true", help="vertex colours from the model, seen head-on")
+    p.add_argument("--no_normals", action="store_true", help="leave the normals out of the PLY")
+    p.add_argument("--dense", action="store_true", help="the unculled mesh of the whole lattice (mesh.extract_mesh)")
+    p.add_argument("--out", type=str, default="mesh.ply", help="output PLY path")
+    return p
+
+
+def check_args(args, parser):
+    """the refusals, before torch or CUDA: parser.error() (exit status 2) names the flag"""
+    try:
+        with open(args.ckpt_path, "rb"):
+            pass
+    except OSError as e:
+        parser.error("--ckpt_path %s: cannot be read (%s)" % (args.ckpt_path, e.strerror or e))
+    if not (args.scale > 0 and math.isfinite(args.scale)):
+        parser.error("--scale must be positive")
+    if not 2 <= args.resolution <= 8192:
+        parser.error("--resolution must be in 2..8192")
+    if not (args.threshold > 0 and math.isfinite(args.threshold)):
+        parser.error("--threshold must be positive (the sparse mesh fills culled space with 0)")
+    if args.bounds is not None:
+        lo, hi = args.bounds[:3], args.bounds[3:]
+        if not all(math.isfinite(v) for v in args.bounds) or any(a >= b for a, b in zip(lo, hi)):
+            parser.error("--bounds: every lower corner coordinate must be below the upper one")
+    return args
+
+
+def parse_args(argv=None):
+    parser = get_parser()
+    return check_args(parser.parse_args(argv), parser)
+
+
+def load_model(ckpt_path, scale):
+    """NGP(scale) on the current CUDA device with the checkpoint's weights, density_grid and grid_coords registered
+    as train.run registers them, so the full and the slim checkpoint both load"""
+    import torch
+    from . import train
+    from .models.networks import NGP
+    if not torch.cuda.is_available():
+        raise SystemExit("ngp_pl_b200.export_mesh: no CUDA device (there is no CPU path)")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    model = NGP(scale=scale).to(dev)
+    G = model.grid_size
+    model.register_buffer("density_grid", torch.zeros(model.cascades, G ** 3, device=dev))
+    model.register_buffer("grid_coords", torch.stack(torch.meshgrid(
+        *[torch.arange(G, dtype=torch.int32, device=dev)] * 3, indexing="ij"), -1).reshape(-1, 3))
+    try:
+        train.load_weights(model, ckpt_path)
+    except RuntimeError as e:
+        raise SystemExit("ngp_pl_b200.export_mesh: %s does not fit NGP(scale=%g) (%d cascades of %d^3 cells): %s"
+                         % (ckpt_path, scale, model.cascades, G, str(e).splitlines()[0]))
+    return model
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    import torch
+    from . import mesh
+    model = load_model(args.ckpt_path, args.scale)
+    bounds = None if args.bounds is None else (args.bounds[:3], args.bounds[3:])
+    normals = not args.no_normals
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    if args.dense:
+        m = mesh.extract_mesh(model, args.resolution, bounds, args.threshold, normals=normals, colors=args.colors)
+        stats = None
+    else:
+        m, stats = mesh.extract_mesh_sparse(model, args.resolution, bounds, args.threshold, normals=normals,
+                                            colors=args.colors, return_stats=True)
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    mesh.write_ply(args.out, **m)
+    line = "ngp_pl_b200.export_mesh: %s: %d vertices, %d triangles at %d^3 in %.3f s" % (
+        args.out, m["vertices"].shape[0], m["triangles"].shape[0], args.resolution, dt)
+    if stats is not None:
+        line += " (bricks: %d active, %d visited, %d surface)" % (stats["active"], stats["visited"], stats["surface"])
+    print(line, flush=True)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -4,6 +4,9 @@ PyMCubes, trimesh or scikit-image.
     density_volume(model, resolution, bounds=None)                σ on a lattice, (n0, n1, n2) fp32 on the device
     marching_cubes(volume, iso, lo=None, step=None, normals=False) indexed mesh of a σ volume, on the device
     extract_mesh(model, resolution=256, bounds=None, threshold=20.0, normals=True, colors=False)
+    occupied_bricks(model, resolution, bounds=None)               brick mask of the occupancy grid, bool on the device
+    extract_mesh_sparse(model, resolution=1024, bounds=None, threshold=20.0, normals=True, colors=False,
+                        return_stats=False)                       the mesh of σ where the occupancy grid allows a surface
     write_ply(path, vertices, triangles, normals=None, colors=None) binary little-endian PLY, numpy only
 
 The σ lattice is evaluated by `ngp_density_lattice` (csrc/network.cu), which generates its points instead of reading
@@ -11,6 +14,10 @@ them, and the mesh by `ngp_marching_cubes_count` / `_emit` (csrc/mesh.cu), which
 semantics in include/ngp_b200.h. The only host synchronisations are the read-back of the vertex and triangle counts
 and emit's check of the capacities against them. Model and volume must live on a CUDA device, otherwise RuntimeError;
 there is no CPU path.
+
+The sparse path (`ngp_mesh_brick_mask`, `ngp_mesh_sparse_*` in csrc/mesh.cu) cuts the lattice into bricks of 8^3
+points, evaluates σ only on the bricks near occupied cells of `model.density_bitfield` and keeps σ in memory only for
+the bricks a surface passes through; its cost and memory follow the occupied volume and the surface, not N^3.
 """
 import ctypes as C
 
@@ -148,16 +155,119 @@ def extract_mesh(model, resolution=256, bounds=None, threshold=20.0, normals=Tru
     lat = lattice(resolution, lo, hi)
     sigma = _density(model, lat)
     verts, tris, nrm = _mc(sigma, threshold, lat, normals or colors)
-    rgb = None
-    if colors:
-        d = -nrm
-        flat = (nrm == 0).all(1)
-        d[flat] = torch.tensor([0.0, 0.0, 1.0], device=d.device)
-        rgb = torch.empty(0, 3, device=verts.device, dtype=torch.uint8)
-        if verts.shape[0] > 0:
-            _, c = model(verts, d)
-            rgb = (c.float() * 255).round().clamp(0, 255).to(torch.uint8)
+    rgb = _vertex_colors(model, verts, nrm) if colors else None
     return {"vertices": verts, "triangles": tris, "normals": nrm if normals else None, "colors": rgb}
+
+
+def _vertex_colors(model, verts, nrm):
+    """rgb of model(verts, -nrm) as uint8; a vertex with a zero normal is seen along -z"""
+    d = -nrm
+    flat = (nrm == 0).all(1)
+    d[flat] = torch.tensor([0.0, 0.0, 1.0], device=d.device)
+    rgb = torch.empty(0, 3, device=verts.device, dtype=torch.uint8)
+    if verts.shape[0] > 0:
+        _, c = model(verts, d)
+        rgb = (c.float() * 255).round().clamp(0, 255).to(torch.uint8)
+    return rgb
+
+
+def _brick_mask(model, lat):
+    """the brick bitmask (int32 words) of lattice `lat` over the model's occupancy bitfield"""
+    dev = model.density_bitfield.device
+    _chk(model.density_bitfield, "occupied_bricks")
+    G, C_ = int(model.grid_size), int(model.cascades)
+    if model.density_bitfield.numel() * 8 != C_ * G ** 3:
+        raise RuntimeError("ngp_pl_b200.mesh: density_bitfield has %d bytes, %d cascades of %d^3 cells need %d"
+                           % (model.density_bitfield.numel(), C_, G, C_ * G ** 3 // 8))
+    L = _lib.lib()
+    nbytes = L.ngp_mesh_bricks_bytes(C.byref(lat))
+    if nbytes == 0:
+        raise RuntimeError("ngp_pl_b200.mesh: the sparse path takes 2..%d points per axis, got %s"
+                           % (_lib.NGP_MESH_MAX_N, tuple(lat.n)))
+    mask = torch.empty(nbytes // 4, device=dev, dtype=torch.int32)
+    with torch.cuda.device(dev):
+        _lib.check(L.ngp_mesh_brick_mask(model.density_bitfield.contiguous().data_ptr(), C_, G, float(model.scale),
+                                         C.byref(lat), mask.data_ptr(), _st(dev)), "ngp_mesh_brick_mask")
+    return mask
+
+
+@torch.no_grad()
+def occupied_bricks(model, resolution, bounds=None):
+    """(nb0, nb1, nb2) bool CUDA tensor, nb = ceil(n / 8): the bricks of 8^3 lattice points (lattice as in
+    density_volume) near an occupied cell of model.density_bitfield -- the rule of include/ngp_b200.h (brick mask)"""
+    _chk(model.xyz_encoder.params, "occupied_bricks")
+    lo, hi = _bounds(model, bounds)
+    lat = lattice(resolution, lo, hi)
+    words = _brick_mask(model, lat)
+    B = _lib.NGP_MESH_BRICK
+    nb = [(lat.n[a] + B - 1) // B for a in range(3)]
+    bits = (words.view(-1, 1) >> torch.arange(32, device=words.device, dtype=torch.int32)) & 1
+    return bits.reshape(-1)[:nb[0] * nb[1] * nb[2]].bool().reshape(nb)
+
+
+def _free_bytes(dev):
+    free, _ = torch.cuda.mem_get_info(dev)
+    return free + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+
+
+def _need(dev, nbytes, what):
+    if nbytes > _free_bytes(dev):
+        raise RuntimeError("ngp_pl_b200.mesh.extract_mesh_sparse: %s need %d bytes of device memory, %d are free"
+                           % (what, nbytes, _free_bytes(dev)))
+
+
+@torch.no_grad()
+def extract_mesh_sparse(model, resolution=1024, bounds=None, threshold=20.0, normals=True, colors=False,
+                        return_stats=False):
+    """The mesh of σ_masked at `threshold`: σ at the points of the bricks occupied_bricks() marks, 0 elsewhere. Returns
+    exactly what marching_cubes(σ_masked, threshold) with world-space vertices returns -- the same vertices in the same
+    order, triangles and normals, bitwise -- and colours as extract_mesh computes them; the same dict keys as
+    extract_mesh. Where the occupancy grid is empty the surface is closed, so the mesh stays watertight. It is not
+    extract_mesh's mesh: a surface extract_mesh finds away from occupied cells is not here.
+
+    resolution: 2..8192 points per axis (int or 3 ints); threshold must be > 0. σ is stored only for the bricks a surface
+    passes through; RuntimeError, before allocating, when those bricks or the output do not fit in free device memory.
+    return_stats=True also returns {'active', 'visited', 'surface'} brick counts."""
+    _chk(model.xyz_encoder.params, "extract_mesh_sparse")
+    if not threshold > 0:
+        raise RuntimeError("ngp_pl_b200.mesh.extract_mesh_sparse: threshold must be > 0, got %r" % (threshold,))
+    lo, hi = _bounds(model, bounds)
+    lat = lattice(resolution, lo, hi)
+    dev = model.xyz_encoder.params.device
+    L = _lib.lib()
+    iso = float(threshold)
+    with torch.cuda.device(dev):
+        mask = _brick_mask(model, lat)
+        net, keep = _net_struct(model)
+        st = _st(dev)
+        ws_bytes = L.ngp_mesh_sparse_workspace(C.byref(lat))
+        ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+        bc = (C.c_int64 * 3)()
+        _lib.check(L.ngp_mesh_sparse_bricks(C.byref(net), C.byref(lat), iso, mask.data_ptr(), bc, ws.data_ptr(), ws_bytes,
+                                            st), "ngp_mesh_sparse_bricks")
+        n_surf = int(bc[2])
+        sf_bytes = L.ngp_mesh_surface_workspace(C.byref(lat), n_surf)
+        _need(dev, sf_bytes, "%d surface bricks" % n_surf)
+        sf = torch.empty(sf_bytes, device=dev, dtype=torch.uint8)
+        tot = (C.c_int64 * 2)()
+        _lib.check(L.ngp_mesh_sparse_count(C.byref(net), C.byref(lat), iso, mask.data_ptr(), n_surf, tot, ws.data_ptr(),
+                                           ws_bytes, sf.data_ptr(), sf_bytes, st), "ngp_mesh_sparse_count")
+        del ws
+        nv, nt = int(tot[0]), int(tot[1])
+        want_n = normals or colors
+        _need(dev, nv * 12 * (2 if want_n else 1) + nt * 24, "%d vertices and %d triangles" % (nv, nt))
+        verts = torch.empty(nv, 3, device=dev, dtype=torch.float32)
+        tris = torch.empty(nt, 3, device=dev, dtype=torch.int64)
+        nrm = torch.empty(nv, 3, device=dev, dtype=torch.float32) if want_n else None
+        if nv > 0:
+            _lib.check(L.ngp_mesh_sparse_emit(C.byref(lat), iso, n_surf, verts.data_ptr(), nrm.data_ptr() if want_n else None,
+                                              tris.data_ptr(), nv, nt, sf.data_ptr(), sf_bytes, st), "ngp_mesh_sparse_emit")
+        del sf
+    rgb = _vertex_colors(model, verts, nrm) if colors else None
+    m = {"vertices": verts, "triangles": tris, "normals": nrm if normals else None, "colors": rgb}
+    if return_stats:
+        return m, {"active": int(bc[0]), "visited": int(bc[1]), "surface": n_surf}
+    return m
 
 
 def _np(a):

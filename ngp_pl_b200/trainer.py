@@ -15,6 +15,7 @@ inside the Adam kernel (grad_mul = 1/world_size). The occupancy bitfield is refr
 from identical parameters and then broadcast from rank 0 so all ranks march the same grid.
 """
 import ctypes as C
+import gc
 import math
 
 import torch
@@ -687,8 +688,17 @@ class Trainer:
         g = torch.cuda.CUDAGraph()
         g.register_generator_state(self.gen)
         n0 = int(_lib.lib().ngp_launch_count())
-        with torch.cuda.graph(g):
-            fn()
+        # No automatic garbage collection while capturing: torch.cuda.graph no longer collects before it begins, so a
+        # dead object cycle holding CUDA graphs (a deleted Trainer's) could be collected in the middle of the capture,
+        # where destroying a graph is not permitted and invalidates the capture. The cycle is collected afterwards.
+        gc_was_enabled = gc.isenabled()
+        gc.disable()
+        try:
+            with torch.cuda.graph(g):
+                fn()
+        finally:
+            if gc_was_enabled:
+                gc.enable()
         self._graph_nodes[id(g)] = int(_lib.lib().ngp_launch_count()) - n0
         return g
 
