@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 9
+#define NGP_ABI_VERSION 10
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -683,6 +683,57 @@ int ngp_mesh_sparse_count(const NgpNet* net, const NgpLattice* lat, float iso, c
 int ngp_mesh_sparse_emit(const NgpLattice* lat, float iso, int64_t n_surface, float* vertices, float* normals,
                          int64_t* triangles, int64_t max_vertices, int64_t max_triangles, void* surface_ws,
                          size_t surface_bytes, void* stream);
+
+/* Mesh simplification: vertex clustering with quadric-error placement (Lindstrom, "Out-of-core simplification of large
+ * polygonal models", SIGGRAPH 2000). Input: V vertices (V, 3) fp32, F triangles (F, 3) int64, optional normals (V, 3)
+ * fp32 and colours (V, 3) uint8. numpy float64 restatement: oracle/mesh_simplify.py.
+ *   1. Cluster grid (computed on the host in fp32 from bounds lo < hi and grid g in 1..65536): cubes of side
+ *      h = max_a(hi_a - lo_a) / g, n_a = min(g, max(1, ceil((hi_a - lo_a) / h))) cells on axis a. Vertex cell
+ *      c_a = clamp(floor(__fdiv_rn(__fsub_rn(v_a, lo_a), h)), 0, n_a - 1) -- vertices outside the bounds clamp to the
+ *      border cells -- and cluster key (c0*n1 + c1)*n2 + c2 (int64). A cluster is the set of vertices of one key.
+ *   2. Quadrics: per triangle, in double, n_t = (v1 - v0) x (v2 - v0) of the fp32 positions, area = |n_t| / 2,
+ *      u = n_t / |n_t|, d = -u.v0; area * [u; d][u; d]^T is added to the cluster of each of its three corners (a cluster
+ *      holding two corners gets it twice), collapsing triangles included; |n_t| = 0 contributes nothing. Evaluated in
+ *      the cell-local coordinates of the receiving cluster (origin lo + c * h), which leaves A unchanged.
+ *   3. Representative: x_bar = mean of the cluster's vertices, A and b of its summed quadric (error x^T A x + 2 b^T x +
+ *      c); with A's eigenpairs (lambda_i, e_i), x = x_bar - sum over lambda_i > 1e-3 * lambda_max of
+ *      e_i (e_i^T (A x_bar + b)) / lambda_i (x = x_bar when lambda_max = 0); clamped to the axis-aligned box of the
+ *      cluster's vertices and rounded to fp32. Every vertex therefore lies within sqrt(3) * h of its representative.
+ *      The eigensolve is NGP_SIMPLIFY_JACOBI_SWEEPS cyclic Jacobi sweeps in double.
+ *   4. Normals: the normalised double sum of the cluster's input normals, exactly 0 when that sum is 0. Colours:
+ *      floor(mean + 1/2) per channel, from exact integer sums.
+ *   5. Triangles: each maps to its three cluster keys; one with two equal keys is dropped; of triangles whose key
+ *      triples are the same cyclic rotation, only the first in input order is kept (opposite orientations are both
+ *      kept: the result need not be manifold). Kept triangles stay in input order, with their corner order.
+ *   6. Vertices: one per cluster referenced by a kept triangle, in ascending key order, numbered 0..V'-1.
+ *   7. Determinism: sorted segment reductions in a fixed order (radix sorts, then lane-strided sums and a fixed shuffle
+ *      tree per segment), no float atomics: two calls are bitwise equal.
+ * ngp_mesh_simplify_count computes clusters, quadrics, representatives and kept triangles into the workspace and writes
+ * {V', F'} to the host int64[2] `counts` (one read-back: the call synchronises the stream). Triangle indices are
+ * checked on the device: an index outside [0, V) makes count return NGP_EINVAL (the kernels never read through it).
+ * ngp_mesh_simplify_emit, with the same triangles, V, F and workspace and nothing else touching the workspace in
+ * between, checks max_vertices / max_triangles against {V', F'} (a read-back; NGP_EINVAL with nothing written when
+ * short) and writes out_vertices (V', 3) fp32, out_triangles (F', 3) int64, and out_normals (V', 3) fp32 / out_colors
+ * (V', 3) uint8 where both that input and that output pointer are non-NULL.
+ * ngp_mesh_simplify_workspace(V, F) is about 52 V + 52 F bytes plus cub's temporary storage (sort keys and ids of the
+ * vertices and of the 3F corners), or 0 for V or F outside [0, 2^31). Both calls return NGP_EINVAL for V or F outside
+ * [0, 2^31), a NULL pointer that is needed or a short workspace, and count also for a grid with n_a outside
+ * 1..NGP_SIMPLIFY_MAX_GRID or h not positive and finite. V = 0 or F = 0 gives an empty mesh. */
+#define NGP_SIMPLIFY_MAX_GRID 65536
+#define NGP_SIMPLIFY_JACOBI_SWEEPS 8
+typedef struct {
+    float lo[3];
+    float h;
+    int32_t n[3];
+} NgpClusterGrid;
+size_t ngp_mesh_simplify_workspace(int64_t n_vertices, int64_t n_triangles);
+int ngp_mesh_simplify_count(const float* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
+                            const NgpClusterGrid* grid, int64_t* counts, void* workspace, size_t workspace_bytes,
+                            void* stream);
+int ngp_mesh_simplify_emit(const int64_t* triangles, int64_t n_vertices, int64_t n_triangles, const float* normals,
+                           const uint8_t* colors, float* out_vertices, float* out_normals, uint8_t* out_colors,
+                           int64_t* out_triangles, int64_t max_vertices, int64_t max_triangles, void* workspace,
+                           size_t workspace_bytes, void* stream);
 
 /* ----------------------------------------------------------------------------------------------
  * Test-view images of the validation pass (reference train.py:215-221): `{idx:03d}.png` holds (rgb_pred*255).astype(np.uint8)

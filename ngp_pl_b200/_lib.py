@@ -9,7 +9,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 9  #NGP_ABI_VERSION in include/ngp_b200.h
+ABI_VERSION = 10  #NGP_ABI_VERSION in include/ngp_b200.h
 
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
@@ -18,6 +18,7 @@ NGP_MC_SLAB_POINTS = 1 << 20
 NGP_MESH_BRICK = 8
 NGP_MESH_MAX_N = 8192
 NGP_MESH_CHUNK_BRICKS = 1 << 16
+NGP_SIMPLIFY_MAX_GRID = 65536
 NGP_VIEW_IMAGES_WORKSPACE = 4096
 NGP_PNG_FIXED = 0
 NGP_PNG_DYNAMIC = 1
@@ -70,6 +71,15 @@ class NgpLattice(C.Structure):
         ("n", C.c_int32 * 3),
         ("lo", C.c_float * 3),
         ("step", C.c_float * 3),
+    ]
+
+
+class NgpClusterGrid(C.Structure):
+    """Mirror of NgpClusterGrid in include/ngp_b200.h."""
+    _fields_ = [
+        ("lo", C.c_float * 3),
+        ("h", C.c_float),
+        ("n", C.c_int32 * 3),
     ]
 
 
@@ -214,6 +224,9 @@ SIGNATURES = {
     "ngp_mesh_surface_workspace": (_sz, [C.POINTER(NgpLattice), _i64]),
     "ngp_mesh_sparse_count": (_i, [C.POINTER(NgpNet), C.POINTER(NgpLattice), _f, _P, _i64, _P, _P, _sz, _P, _sz, _P]),
     "ngp_mesh_sparse_emit": (_i, [C.POINTER(NgpLattice), _f, _i64, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
+    "ngp_mesh_simplify_workspace": (_sz, [_i64, _i64]),
+    "ngp_mesh_simplify_count": (_i, [_P, _i64, _P, _i64, C.POINTER(NgpClusterGrid), _P, _P, _sz, _P]),
+    "ngp_mesh_simplify_emit": (_i, [_P, _i64, _i64, _P, _P, _P, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
     "ngp_view_images": (_i, [_P, _P, _i, _i, _P, _P, _P, _sz, _P]),
     "ngp_png_workspace": (_sz, [_i, _i]),
     "ngp_png_capacity": (_sz, [_i, _i]),

@@ -1,12 +1,15 @@
 """Export the mesh of a trained checkpoint as a binary PLY.
 
     python -m ngp_pl_b200.export_mesh --ckpt_path ckpts/nsvf/Lego/epoch=29.ckpt [--scale 0.5] [--resolution 1024]
-        [--threshold 20] [--bounds x0 y0 z0 x1 y1 z1] [--colors] [--no_normals] [--dense] [--out mesh.ply]
+        [--threshold 20] [--bounds x0 y0 z0 x1 y1 z1] [--colors] [--no_normals] [--dense] [--simplify G]
+        [--out mesh.ply]
 
 The checkpoint is the full or the slim one train.py writes; it is loaded into NGP(scale) with train.load_weights. By
 default the mesh is mesh.extract_mesh_sparse's: σ evaluated and marching cubes run only near the cells the model's
 occupancy grid marks, so 2048^3 and 4096^3 lattices fit in memory. --dense gives mesh.extract_mesh's mesh of the whole
 lattice (the notebook's mesh cell): a different mesh, which also has the surfaces the occupancy grid has culled.
+--simplify G then reduces the mesh with mesh.simplify_mesh on a G^3 cluster grid over the lattice box (vertex
+clustering with quadric-error placement; colours become the means of each cluster's colours).
 Bad arguments are refused with exit status 2 before torch is imported.
 """
 import argparse
@@ -27,6 +30,8 @@ def get_parser():
     p.add_argument("--colors", action="store_true", help="vertex colours from the model, seen head-on")
     p.add_argument("--no_normals", action="store_true", help="leave the normals out of the PLY")
     p.add_argument("--dense", action="store_true", help="the unculled mesh of the whole lattice (mesh.extract_mesh)")
+    p.add_argument("--simplify", type=int, default=None, metavar="G",
+                   help="simplify on a G^3 cluster grid over the lattice box before writing, 1..65536")
     p.add_argument("--out", type=str, default="mesh.ply", help="output PLY path")
     return p
 
@@ -48,6 +53,8 @@ def check_args(args, parser):
         lo, hi = args.bounds[:3], args.bounds[3:]
         if not all(math.isfinite(v) for v in args.bounds) or any(a >= b for a, b in zip(lo, hi)):
             parser.error("--bounds: every lower corner coordinate must be below the upper one")
+    if args.simplify is not None and not 1 <= args.simplify <= 65536:
+        parser.error("--simplify must be in 1..65536")
     return args
 
 
@@ -95,11 +102,18 @@ def main(argv=None):
                                             colors=args.colors, return_stats=True)
     torch.cuda.synchronize()
     dt = time.perf_counter() - t0
-    mesh.write_ply(args.out, **m)
     line = "ngp_pl_b200.export_mesh: %s: %d vertices, %d triangles at %d^3 in %.3f s" % (
         args.out, m["vertices"].shape[0], m["triangles"].shape[0], args.resolution, dt)
     if stats is not None:
         line += " (bricks: %d active, %d visited, %d surface)" % (stats["active"], stats["visited"], stats["surface"])
+    if args.simplify is not None:
+        box = bounds if bounds is not None else (model._xyz_min_host, model._xyz_max_host)
+        t0 = time.perf_counter()
+        m = mesh.simplify_mesh(m, args.simplify, box)
+        torch.cuda.synchronize()
+        line += "; simplified at grid %d to %d vertices, %d triangles in %.3f s" % (
+            args.simplify, m["vertices"].shape[0], m["triangles"].shape[0], time.perf_counter() - t0)
+    mesh.write_ply(args.out, **m)
     print(line, flush=True)
     return 0
 

@@ -7,6 +7,7 @@ PyMCubes, trimesh or scikit-image.
     occupied_bricks(model, resolution, bounds=None)               brick mask of the occupancy grid, bool on the device
     extract_mesh_sparse(model, resolution=1024, bounds=None, threshold=20.0, normals=True, colors=False,
                         return_stats=False)                       the mesh of σ where the occupancy grid allows a surface
+    simplify_mesh(mesh, grid, bounds=None)                        vertex clustering with quadric-error placement
     write_ply(path, vertices, triangles, normals=None, colors=None) binary little-endian PLY, numpy only
 
 The σ lattice is evaluated by `ngp_density_lattice` (csrc/network.cu), which generates its points instead of reading
@@ -18,6 +19,10 @@ there is no CPU path.
 The sparse path (`ngp_mesh_brick_mask`, `ngp_mesh_sparse_*` in csrc/mesh.cu) cuts the lattice into bricks of 8^3
 points, evaluates σ only on the bricks near occupied cells of `model.density_bitfield` and keeps σ in memory only for
 the bricks a surface passes through; its cost and memory follow the occupied volume and the surface, not N^3.
+
+simplify_mesh (`ngp_mesh_simplify_count` / `_emit`) reduces a mesh to at most one vertex per cell of a grid^3 cluster
+grid, placed where the cell's triangle planes meet (quadric error), so thin parts and sharp edges a coarser lattice
+would lose keep their place at a fraction of the triangle count.
 """
 import ctypes as C
 
@@ -210,10 +215,10 @@ def _free_bytes(dev):
     return free + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
 
 
-def _need(dev, nbytes, what):
+def _need(dev, nbytes, what, fn="extract_mesh_sparse"):
     if nbytes > _free_bytes(dev):
-        raise RuntimeError("ngp_pl_b200.mesh.extract_mesh_sparse: %s need %d bytes of device memory, %d are free"
-                           % (what, nbytes, _free_bytes(dev)))
+        raise RuntimeError("ngp_pl_b200.mesh.%s: %s need %d bytes of device memory, %d are free"
+                           % (fn, what, nbytes, _free_bytes(dev)))
 
 
 @torch.no_grad()
@@ -268,6 +273,95 @@ def extract_mesh_sparse(model, resolution=1024, bounds=None, threshold=20.0, nor
     if return_stats:
         return m, {"active": int(bc[0]), "visited": int(bc[1]), "surface": n_surf}
     return m
+
+
+def cluster_grid(lo, hi, grid):
+    """NgpClusterGrid of rule 1 (include/ngp_b200.h), in fp32: h = max(hi - lo) / grid, n = min(grid, max(1,
+    ceil((hi - lo) / h))) cells per axis"""
+    lo = _three(lo, np.float32)
+    ext = _three(hi, np.float32) - lo
+    h = np.float32(ext.max() / np.float32(grid))
+    n = np.minimum(np.maximum(1, np.ceil(ext / h).astype(np.int64)), int(grid))
+    g = _lib.NgpClusterGrid()
+    for a in range(3):
+        g.lo[a], g.n[a] = float(lo[a]), int(n[a])
+    g.h = float(h)
+    return g
+
+
+@torch.no_grad()
+def simplify_mesh(mesh, grid, bounds=None):
+    """Vertex clustering with quadric-error placement (Lindstrom 2000; the rule is in include/ngp_b200.h) of a mesh
+    dict as extract_mesh / extract_mesh_sparse return it: at most one vertex per cell of a cluster grid of cubes of side
+    max(hi - lo) / grid over `bounds` = (lo, hi), placed at the least quadric error of the cell's triangle planes
+    within the box of the cell's vertices. Triangles whose corners fall in fewer than three cells are dropped, and so
+    is every later triangle with the same cells in the same cyclic order; the mesh need not stay manifold. Returns a
+    dict with the same keys: normals are the normalised sums of the cell's normals and colours the rounded means of its
+    colours, None where the input's are. Vertices outside the bounds join the border cells.
+
+    grid: 1..65536. bounds=None: the bounding box of the vertices (one device min / max and its read-back). RuntimeError,
+    before allocating, for CPU tensors, a grid out of range, lo >= hi on an axis, or a workspace or output that does
+    not fit in free device memory. Deterministic: two calls are bitwise equal."""
+    verts, tris = mesh["vertices"], mesh["triangles"]
+    nrm, col = mesh.get("normals"), mesh.get("colors")
+    for t, what in ((verts, "vertices"), (tris, "triangles"), (nrm, "normals"), (col, "colors")):
+        if t is not None:
+            _chk(t, "simplify_mesh")
+    if isinstance(grid, bool) or not isinstance(grid, (int, np.integer)) or not 1 <= grid <= _lib.NGP_SIMPLIFY_MAX_GRID:
+        raise RuntimeError("ngp_pl_b200.mesh.simplify_mesh: grid must be an integer in 1..%d, got %r"
+                           % (_lib.NGP_SIMPLIFY_MAX_GRID, grid))
+    dev = verts.device
+    verts = verts.detach().to(torch.float32).reshape(-1, 3).contiguous()
+    tris = tris.detach().to(torch.int64).reshape(-1, 3).contiguous()
+    V, F = verts.shape[0], tris.shape[0]
+    if nrm is not None:
+        nrm = nrm.detach().to(torch.float32).reshape(-1, 3).contiguous()
+    if col is not None:
+        col = col.detach().to(torch.uint8).reshape(-1, 3).contiguous()
+    for t, what in ((nrm, "normals"), (col, "colors")):
+        if t is not None and t.shape[0] != V:
+            raise RuntimeError("ngp_pl_b200.mesh.simplify_mesh: %d %s for %d vertices" % (t.shape[0], what, V))
+    if bounds is None:
+        if V == 0:
+            lo, hi = np.zeros(3, np.float32), np.ones(3, np.float32)
+        else:
+            mn, mx = torch.aminmax(verts, dim=0)
+            lo, hi = mn.cpu().numpy(), mx.cpu().numpy()
+            if not (hi - lo).max() > 0:
+                raise RuntimeError("ngp_pl_b200.mesh.simplify_mesh: the vertices span no volume (%s .. %s); pass bounds"
+                                   % (lo, hi))
+    else:
+        lo, hi = (_np(b).astype(np.float32).reshape(-1) for b in bounds)
+        lo, hi = _three(lo, np.float32), _three(hi, np.float32)
+        if not (np.isfinite(lo).all() and np.isfinite(hi).all() and (lo < hi).all()):
+            raise RuntimeError("ngp_pl_b200.mesh.simplify_mesh: bounds need lo < hi on every axis, got %s .. %s" % (lo, hi))
+    g = cluster_grid(lo, hi, int(grid))
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        ws_bytes = L.ngp_mesh_simplify_workspace(V, F)
+        if ws_bytes == 0:
+            raise RuntimeError("ngp_pl_b200.mesh.simplify_mesh: %d vertices and %d triangles: both must be below 2^31"
+                               % (V, F))
+        _need(dev, ws_bytes, "the workspace of %d vertices and %d triangles" % (V, F), "simplify_mesh")
+        ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+        st = _st(dev)
+        tot = (C.c_int64 * 2)()
+        _lib.check(L.ngp_mesh_simplify_count(verts.data_ptr(), V, tris.data_ptr(), F, C.byref(g), tot, ws.data_ptr(),
+                                             ws_bytes, st), "ngp_mesh_simplify_count")
+        nv, nt = int(tot[0]), int(tot[1])
+        _need(dev, nv * (12 + (12 if nrm is not None else 0) + (3 if col is not None else 0)) + nt * 24,
+              "%d vertices and %d triangles" % (nv, nt), "simplify_mesh")
+        out_v = torch.empty(nv, 3, device=dev, dtype=torch.float32)
+        out_t = torch.empty(nt, 3, device=dev, dtype=torch.int64)
+        out_n = torch.empty(nv, 3, device=dev, dtype=torch.float32) if nrm is not None else None
+        out_c = torch.empty(nv, 3, device=dev, dtype=torch.uint8) if col is not None else None
+        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        if nv > 0:
+            _lib.check(L.ngp_mesh_simplify_emit(tris.data_ptr(), V, F, ptr(nrm), ptr(col), out_v.data_ptr(), ptr(out_n),
+                                                ptr(out_c), out_t.data_ptr(), nv, nt, ws.data_ptr(), ws_bytes, st),
+                       "ngp_mesh_simplify_emit")
+        del ws
+    return {"vertices": out_v, "triangles": out_t, "normals": out_n, "colors": out_c}
 
 
 def _np(a):
