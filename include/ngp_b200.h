@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 10
+#define NGP_ABI_VERSION 11
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -734,6 +734,76 @@ int ngp_mesh_simplify_emit(const int64_t* triangles, int64_t n_vertices, int64_t
                            const uint8_t* colors, float* out_vertices, float* out_normals, uint8_t* out_colors,
                            int64_t* out_triangles, int64_t max_vertices, int64_t max_triangles, void* workspace,
                            size_t workspace_bytes, void* stream);
+
+/* Texture baking: a per-triangle texture atlas of side W (a power of two in [16, 16384]) and its colours from the model.
+ * Input: V vertices (V, 3) fp32, F triangles (F, 3) int64 (counter-clockwise seen from outside), optional normals
+ * (V, 3) fp32. Margin m = 1 texel, smallest square s_min = 4. numpy float64 restatement: oracle/mesh_texture.py.
+ *   1. Longest edge, in double on the fp32 positions: the edge lengths |b-a|, |c-b|, |a-c| of corners (a, b, c); the
+ *      first maximum is the longest. The corners rotated so that it runs from the first to the second are A, B, C (the
+ *      same cyclic order). l = |B - A|, frexp(l) = f * 2^e with f in [1/2, 1); e_top = max e over the triangles with
+ *      l > 0 and finite; class k = min(e_top - e, 63), and k = 63 for l = 0 or not finite.
+ *   2. Square side s = max(s_min, S >> k) (0 for k >= 31, so s_min), S the largest power of two in [s_min, W] with
+ *      sum s^2 <= W^2, found on the host from a device histogram of the classes (64 bins, one read-back). F s_min^2 > W^2
+ *      is refused.
+ *   3. Packing: the squares ordered by s descending, ties by triangle index. Square i's Morton offset is the exclusive
+ *      sum of s^2 before it; its lower-left texel (x0, y0) is that offset with x in the even bits and y in the odd bits
+ *      (y from the bottom). Every earlier square is at least as large and every area a power of 4 times s^2, so each
+ *      square is an aligned s x s block and no two overlap. Texel (x, y) has atlas index m = interleave(x, y), the same
+ *      Morton code, so square i holds the atlas indices [offset_i, offset_i + s_i^2).
+ *   4. Placement, a similarity transform, in double and rounded to fp32 once: rho = (s - 2m) / 2^e texels per world
+ *      unit, u = (B - A) / l, w = (C - A).u, eta = |(C - A) - w u|; A' = (x0 + m, y0 + m), B' = A' + (rho l, 0),
+ *      C' = A' + rho (w, eta) (A' = B' = C' for l = 0 or not finite). uv (F, 3, 2) lists the corners in the triangle's
+ *      own order. AB is the longest edge, so 0 <= w <= l, eta < l: the triangle keeps m texels from the square's sides
+ *      and stays counter-clockwise.
+ *   5. Band: texel (x, y) of triangle i's square is baked when the open box (x + 1/2 +- 1, y + 1/2 +- 1) meets the
+ *      closed uv triangle (every texel bilinear filtering of a point of the triangle reads): separating-axis tests in
+ *      double on the fp32 uv along x, y and the normals of the triangle's non-zero edges, an axis separating when the
+ *      triangle's interval [lo, hi] has hi <= box_lo or lo >= box_hi. Every other texel of the atlas is (0, 0, 0).
+ *      A baked texel maps to the closest point of the uv triangle to its centre (the interior when the centre is inside
+ *      a triangle of non-zero area, else the nearest of the clamped projections onto AB, BC, CA, the first on a tie), in
+ *      double; its barycentrics give p = A + bB (B - A) + bC (C - A) and n = the normalised bA nA + bB nB + bC nC when
+ *      the mesh has normals and that mix is non-zero, else the normalised (B - A) x (C - A), else (0, 0, -1); both are
+ *      rounded to fp32. The texel map lists the baked texels in ascending atlas index.
+ *   6. Bake, K samples (1..256) from offset r >= 0, all fp32: o = fmaf(n, r, p), d = -n, delta = (2r) / K,
+ *      t_j = (j + 1/2) delta for j < K, t_K = r, x_j = fmaf(d, t_j, o) -- ngp_net_forward's ray mode, which evaluates
+ *      (sigma_j, c_j) = NGP.forward(x_j, d). Composite in double: T_0 = 1, alpha_j = 1 - exp(-sigma_j delta),
+ *      T_{j+1} = T_j (1 - alpha_j), C = sum_{j<K} T_j alpha_j c_j + T_K c_K (the surface's own colour is the background);
+ *      texel = rint(255 C) clamped to [0, 255]. r = 0 gives rint(255 NGP.forward(p, d)). Image row W - 1 - y holds
+ *      texel row y.
+ * No float atomics: two calls are bitwise equal.
+ *
+ * ngp_mesh_texture_atlas: steps 1-5 up to the band count. Writes uv, squares (F, 3) int32 (x0, y0, s), and {S, number
+ * of band texels} to the host int64[2] `counts` (two read-backs: the call synchronises the stream). Triangle indices are
+ * checked on the device: an index outside [0, V) returns NGP_EINVAL.
+ * ngp_mesh_texture_texels, with the same vertices, triangles, W and workspace and nothing else touching the workspace in
+ * between: the texel map, texel (n) int64 atlas indices, triangle (n) int32, point (n, 3) and normal (n, 3) fp32, with
+ * n = counts[1]; NGP_EINVAL when max_texels < n (a read-back, nothing written).
+ * ngp_mesh_texture_workspace(V, F, W) is about 32 F + 4 W^2 bytes plus cub's temporary storage, or 0 for V or F outside
+ * [0, 2^31) or W not a power of two in [16, 16384]. Both calls return NGP_EINVAL for those sizes, F s_min^2 > W^2, a
+ * NULL pointer that is needed or a short workspace.
+ * ngp_mesh_texture_bake: texture (W, W, 3) uint8 from the texel map (texel, point, normal of n texels), in chunks of
+ * max(1, NGP_TEXTURE_CHUNK_SAMPLES / (K + 1)) texels, so the workspace, ngp_mesh_texture_bake_workspace(K) bytes (0 for
+ * K outside 1..256), grows with one chunk. NGP_EINVAL for a bad size, r negative or not finite, a NULL pointer that is
+ * needed, a short workspace, or a texel index outside [0, W^2) (checked on the device, such a texel is not written; a
+ * read-back at the end, so the call synchronises the stream). */
+#define NGP_TEXTURE_MIN_SIZE 16
+#define NGP_TEXTURE_MAX_SIZE 16384
+#define NGP_TEXTURE_MIN_SQUARE 4
+#define NGP_TEXTURE_MARGIN 1
+#define NGP_TEXTURE_MAX_SAMPLES 256
+#define NGP_TEXTURE_CHUNK_SAMPLES (1 << 22)
+size_t ngp_mesh_texture_workspace(int64_t n_vertices, int64_t n_triangles, int size);
+int ngp_mesh_texture_atlas(const float* vertices, int64_t n_vertices, const int64_t* triangles, int64_t n_triangles,
+                           int size, float* uv, int32_t* squares, int64_t* counts, void* workspace, size_t workspace_bytes,
+                           void* stream);
+int ngp_mesh_texture_texels(const float* vertices, const float* normals, int64_t n_vertices, const int64_t* triangles,
+                            int64_t n_triangles, int size, const float* uv, int64_t max_texels, int64_t* texel,
+                            int32_t* triangle, float* point, float* normal, void* workspace, size_t workspace_bytes,
+                            void* stream);
+size_t ngp_mesh_texture_bake_workspace(int samples);
+int ngp_mesh_texture_bake(const NgpNet* net, int size, int64_t n_texels, const int64_t* texel, const float* point,
+                          const float* normal, float offset, int samples, uint8_t* texture, void* workspace,
+                          size_t workspace_bytes, void* stream);
 
 /* ----------------------------------------------------------------------------------------------
  * Test-view images of the validation pass (reference train.py:215-221): `{idx:03d}.png` holds (rgb_pred*255).astype(np.uint8)

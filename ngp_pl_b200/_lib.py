@@ -9,7 +9,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 10  #NGP_ABI_VERSION in include/ngp_b200.h
+ABI_VERSION = 11  #NGP_ABI_VERSION in include/ngp_b200.h
 
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
@@ -19,6 +19,12 @@ NGP_MESH_BRICK = 8
 NGP_MESH_MAX_N = 8192
 NGP_MESH_CHUNK_BRICKS = 1 << 16
 NGP_SIMPLIFY_MAX_GRID = 65536
+NGP_TEXTURE_MIN_SIZE = 16
+NGP_TEXTURE_MAX_SIZE = 16384
+NGP_TEXTURE_MIN_SQUARE = 4
+NGP_TEXTURE_MARGIN = 1
+NGP_TEXTURE_MAX_SAMPLES = 256
+NGP_TEXTURE_CHUNK_SAMPLES = 1 << 22
 NGP_VIEW_IMAGES_WORKSPACE = 4096
 NGP_PNG_FIXED = 0
 NGP_PNG_DYNAMIC = 1
@@ -227,6 +233,11 @@ SIGNATURES = {
     "ngp_mesh_simplify_workspace": (_sz, [_i64, _i64]),
     "ngp_mesh_simplify_count": (_i, [_P, _i64, _P, _i64, C.POINTER(NgpClusterGrid), _P, _P, _sz, _P]),
     "ngp_mesh_simplify_emit": (_i, [_P, _i64, _i64, _P, _P, _P, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
+    "ngp_mesh_texture_workspace": (_sz, [_i64, _i64, _i]),
+    "ngp_mesh_texture_atlas": (_i, [_P, _i64, _P, _i64, _i, _P, _P, _P, _P, _sz, _P]),
+    "ngp_mesh_texture_texels": (_i, [_P, _P, _i64, _P, _i64, _i, _P, _i64, _P, _P, _P, _P, _P, _sz, _P]),
+    "ngp_mesh_texture_bake_workspace": (_sz, [_i]),
+    "ngp_mesh_texture_bake": (_i, [C.POINTER(NgpNet), _i, _i64, _P, _P, _P, _f, _i, _P, _P, _sz, _P]),
     "ngp_view_images": (_i, [_P, _P, _i, _i, _P, _P, _P, _sz, _P]),
     "ngp_png_workspace": (_sz, [_i, _i]),
     "ngp_png_capacity": (_sz, [_i, _i]),

@@ -15,7 +15,10 @@ INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libngp_b200.so")
 
-SOURCES = ["vren_ops.cu", "network.cu", "train.cu", "infer.cu", "modules.cu", "metrics.cu", "mesh.cu", "lpips.cu", "stage.cu", "images.cu", "jpeg.cu"]
+SOURCES = ["vren_ops.cu", "network.cu", "train.cu", "infer.cu", "modules.cu", "metrics.cu", "mesh.cu", "lpips.cu", "stage.cu", "images.cu", "jpeg.cu",
+           "texture.cu"]
+# texture.cu's double arithmetic must round operation by operation as its numpy restatement (oracle/mesh_texture.py) does
+SOURCE_FLAGS = {"texture.cu": ["-fmad=false"]}
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
@@ -28,6 +31,7 @@ def _digest(paths):
         h.update(p.encode())
         h.update(open(p, "rb").read())
     h.update(" ".join(NVCC_FLAGS).encode())
+    h.update(repr(sorted(SOURCE_FLAGS.items())).encode())
     return h.hexdigest()
 
 
@@ -47,7 +51,7 @@ def build(force=False, verbose=False):
 
     def compile_one(src):
         obj = os.path.join(OBJ, os.path.basename(src) + ".o")
-        cmd = ["nvcc", "-c", src, "-o", obj, "-I", INCLUDE] + NVCC_FLAGS
+        cmd = ["nvcc", "-c", src, "-o", obj, "-I", INCLUDE] + NVCC_FLAGS + SOURCE_FLAGS.get(os.path.basename(src), [])
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)
         log = r.stdout.decode()
         open(obj + ".log", "w").write(log)

@@ -1,8 +1,8 @@
-"""Export the mesh of a trained checkpoint as a binary PLY.
+"""Export the mesh of a trained checkpoint as a binary PLY, or as a textured OBJ.
 
     python -m ngp_pl_b200.export_mesh --ckpt_path ckpts/nsvf/Lego/epoch=29.ckpt [--scale 0.5] [--resolution 1024]
         [--threshold 20] [--bounds x0 y0 z0 x1 y1 z1] [--colors] [--no_normals] [--dense] [--simplify G]
-        [--out mesh.ply]
+        [--texture W [--texture_offset R] [--texture_samples K]] [--out mesh.ply]
 
 The checkpoint is the full or the slim one train.py writes; it is loaded into NGP(scale) with train.load_weights. By
 default the mesh is mesh.extract_mesh_sparse's: σ evaluated and marching cubes run only near the cells the model's
@@ -10,6 +10,10 @@ occupancy grid marks, so 2048^3 and 4096^3 lattices fit in memory. --dense gives
 lattice (the notebook's mesh cell): a different mesh, which also has the surfaces the occupancy grid has culled.
 --simplify G then reduces the mesh with mesh.simplify_mesh on a G^3 cluster grid over the lattice box (vertex
 clustering with quadric-error placement; colours become the means of each cluster's colours).
+--texture W bakes the model's colours into a W x W atlas with mesh.bake_texture and writes --out (which must end in
+.obj) with mesh.write_obj, next to its .mtl and .png. The bake renders --texture_samples samples along each texel's
+inward normal from --texture_offset outside the surface: by default the cluster cell with --simplify, where vertices
+sit up to sqrt(3) cells off the surface they stand for, and the largest lattice step without it.
 Bad arguments are refused with exit status 2 before torch is imported.
 """
 import argparse
@@ -32,7 +36,13 @@ def get_parser():
     p.add_argument("--dense", action="store_true", help="the unculled mesh of the whole lattice (mesh.extract_mesh)")
     p.add_argument("--simplify", type=int, default=None, metavar="G",
                    help="simplify on a G^3 cluster grid over the lattice box before writing, 1..65536")
-    p.add_argument("--out", type=str, default="mesh.ply", help="output PLY path")
+    p.add_argument("--texture", type=int, default=None, metavar="W",
+                   help="bake a W x W texture atlas (a power of two in 16..16384) and write an OBJ + MTL + PNG")
+    p.add_argument("--texture_offset", type=float, default=None, metavar="R",
+                   help="start of the bake's rays outside the surface, world units >= 0 (default: the cluster cell "
+                        "with --simplify, else the largest lattice step)")
+    p.add_argument("--texture_samples", type=int, default=16, metavar="K", help="samples per texel, 1..256")
+    p.add_argument("--out", type=str, default="mesh.ply", help="output PLY path (.obj with --texture)")
     return p
 
 
@@ -55,6 +65,17 @@ def check_args(args, parser):
             parser.error("--bounds: every lower corner coordinate must be below the upper one")
     if args.simplify is not None and not 1 <= args.simplify <= 65536:
         parser.error("--simplify must be in 1..65536")
+    if args.texture is not None:
+        if not (16 <= args.texture <= 16384 and args.texture & (args.texture - 1) == 0):
+            parser.error("--texture must be a power of two in 16..16384")
+        if args.colors:
+            parser.error("--texture and --colors exclude each other: the texture carries the colours")
+        if not args.out.lower().endswith(".obj"):
+            parser.error("--out must end in .obj with --texture")
+    if args.texture_offset is not None and not (args.texture_offset >= 0 and math.isfinite(args.texture_offset)):
+        parser.error("--texture_offset must be >= 0 and finite")
+    if not 1 <= args.texture_samples <= 256:
+        parser.error("--texture_samples must be in 1..256")
     return args
 
 
@@ -85,6 +106,15 @@ def load_model(ckpt_path, scale):
     return model
 
 
+def texture_offset(box, resolution, simplify):
+    """the default --texture_offset: the cluster cell side with --simplify, else the largest lattice step (fp32, as
+    mesh.cluster_grid and mesh.lattice compute them)"""
+    from . import mesh
+    if simplify is not None:
+        return float(mesh.cluster_grid(box[0], box[1], simplify).h)
+    return float(max(mesh.lattice(resolution, box[0], box[1]).step))
+
+
 def main(argv=None):
     args = parse_args(argv)
     import torch
@@ -106,14 +136,26 @@ def main(argv=None):
         args.out, m["vertices"].shape[0], m["triangles"].shape[0], args.resolution, dt)
     if stats is not None:
         line += " (bricks: %d active, %d visited, %d surface)" % (stats["active"], stats["visited"], stats["surface"])
+    box = bounds if bounds is not None else (model._xyz_min_host, model._xyz_max_host)
     if args.simplify is not None:
-        box = bounds if bounds is not None else (model._xyz_min_host, model._xyz_max_host)
         t0 = time.perf_counter()
         m = mesh.simplify_mesh(m, args.simplify, box)
         torch.cuda.synchronize()
         line += "; simplified at grid %d to %d vertices, %d triangles in %.3f s" % (
             args.simplify, m["vertices"].shape[0], m["triangles"].shape[0], time.perf_counter() - t0)
-    mesh.write_ply(args.out, **m)
+    if args.texture is None:
+        mesh.write_ply(args.out, **m)
+    else:
+        r = args.texture_offset
+        if r is None:
+            r = texture_offset(box, args.resolution, args.simplify)
+        t0 = time.perf_counter()
+        tex = mesh.bake_texture(model, m, args.texture, r, args.texture_samples, return_texels=True)
+        torch.cuda.synchronize()
+        S = int(tex["squares"][:, 2].max()) if tex["squares"].shape[0] else args.texture
+        line += "; baked a %d^2 atlas (S = %d, %d texels, offset %.6g, %d samples) in %.3f s" % (
+            args.texture, S, tex["texel"].shape[0], r, args.texture_samples, time.perf_counter() - t0)
+        mesh.write_obj(args.out, m["vertices"], m["triangles"], m["normals"], tex["uv"], tex["texture"])
     print(line, flush=True)
     return 0
 

@@ -8,7 +8,11 @@ PyMCubes, trimesh or scikit-image.
     extract_mesh_sparse(model, resolution=1024, bounds=None, threshold=20.0, normals=True, colors=False,
                         return_stats=False)                       the mesh of σ where the occupancy grid allows a surface
     simplify_mesh(mesh, grid, bounds=None)                        vertex clustering with quadric-error placement
+    bake_texture(model, mesh, size=4096, offset=0.0, samples=16, return_texels=False)
+                                                                  a per-triangle texture atlas and its colours
     write_ply(path, vertices, triangles, normals=None, colors=None) binary little-endian PLY, numpy only
+    write_obj(path, vertices, triangles, normals=None, uv=None, texture=None, png_mode="dynamic")
+                                                                  OBJ [+ MTL + PNG encoded on the device]
 
 The σ lattice is evaluated by `ngp_density_lattice` (csrc/network.cu), which generates its points instead of reading
 them, and the mesh by `ngp_marching_cubes_count` / `_emit` (csrc/mesh.cu), which work through the volume in slabs;
@@ -23,6 +27,10 @@ the bricks a surface passes through; its cost and memory follow the occupied vol
 simplify_mesh (`ngp_mesh_simplify_count` / `_emit`) reduces a mesh to at most one vertex per cell of a grid^3 cluster
 grid, placed where the cell's triangle planes meet (quadric error), so thin parts and sharp edges a coarser lattice
 would lose keep their place at a fraction of the triangle count.
+
+bake_texture (`ngp_mesh_texture_atlas` / `_texels` / `_bake` in csrc/texture.cu) gives every triangle its own square
+of a texture atlas and bakes the model's colours into it through the fused forward, so a simplified mesh keeps the
+detail its few vertices cannot hold; write_obj saves mesh, uv and texture for tools that expect a textured OBJ.
 """
 import ctypes as C
 
@@ -364,8 +372,161 @@ def simplify_mesh(mesh, grid, bounds=None):
     return {"vertices": out_v, "triangles": out_t, "normals": out_n, "colors": out_c}
 
 
+def texture_size_for(n_triangles):
+    """the smallest atlas side that holds n_triangles squares of the smallest size"""
+    W = _lib.NGP_TEXTURE_MIN_SIZE
+    while n_triangles * _lib.NGP_TEXTURE_MIN_SQUARE ** 2 > W * W:
+        W *= 2
+    return W
+
+
+@torch.no_grad()
+def bake_texture(model, mesh, size=4096, offset=0.0, samples=16, return_texels=False):
+    """A texture atlas of side `size` for a mesh dict as extract_mesh / extract_mesh_sparse / simplify_mesh return it,
+    and its colours from the model (the rule is in include/ngp_b200.h). Every triangle gets its own power-of-two square,
+    packed along the Morton curve, with the triangle placed undistorted one texel inside it. Every texel bilinear
+    filtering of a point of a triangle reads is baked: a volume render of `samples` samples along -n from `offset` world
+    units outside the surface point the texel maps to, whose own colour is the background (offset 0: the model's colour
+    at the point, seen head-on). Other texels are 0.
+
+    Returns {'uv': (F, 3, 2) float32 texel coordinates per corner (divide by size for OBJ's vt), 'squares': (F, 3) int32
+    (x0, y0, side), 'texture': (size, size, 3) uint8 (row 0 is the top: texel row y is image row size - 1 - y)} on the
+    model's device; return_texels=True adds the texel map: 'texel' (n,) int64 atlas indices (Morton, x in the even bits,
+    ascending), 'triangle' (n,) int32, 'point' and 'normal' (n, 3) float32.
+
+    size: a power of two in 16..16384 that holds 16 F texels; offset: >= 0 and finite; samples: 1..256. RuntimeError,
+    before allocating, for CPU tensors, a value out of range (a size too small names the one that fits) or memory that
+    is not free; also for a triangle index outside [0, V). Deterministic: two calls are bitwise equal."""
+    verts, tris, nrm = mesh["vertices"], mesh["triangles"], mesh.get("normals")
+    _chk(model.xyz_encoder.params, "bake_texture")
+    for t in (verts, tris, nrm):
+        if t is not None:
+            _chk(t, "bake_texture")
+    W = size
+    if isinstance(W, bool) or not isinstance(W, (int, np.integer)) or not (
+            _lib.NGP_TEXTURE_MIN_SIZE <= W <= _lib.NGP_TEXTURE_MAX_SIZE) or W & (W - 1):
+        raise RuntimeError("ngp_pl_b200.mesh.bake_texture: size must be a power of two in %d..%d, got %r"
+                           % (_lib.NGP_TEXTURE_MIN_SIZE, _lib.NGP_TEXTURE_MAX_SIZE, size))
+    if isinstance(samples, bool) or not isinstance(samples, (int, np.integer)) or not (
+            1 <= samples <= _lib.NGP_TEXTURE_MAX_SAMPLES):
+        raise RuntimeError("ngp_pl_b200.mesh.bake_texture: samples must be an integer in 1..%d, got %r"
+                           % (_lib.NGP_TEXTURE_MAX_SAMPLES, samples))
+    r = float(offset)
+    if not (r >= 0 and np.isfinite(r)):
+        raise RuntimeError("ngp_pl_b200.mesh.bake_texture: offset must be >= 0 and finite, got %r" % (offset,))
+    dev = verts.device
+    verts = verts.detach().to(torch.float32).reshape(-1, 3).contiguous()
+    tris = tris.detach().to(torch.int64).reshape(-1, 3).contiguous()
+    V, F = verts.shape[0], tris.shape[0]
+    if nrm is not None:
+        nrm = nrm.detach().to(torch.float32).reshape(-1, 3).contiguous()
+        if nrm.shape[0] != V:
+            raise RuntimeError("ngp_pl_b200.mesh.bake_texture: %d normals for %d vertices" % (nrm.shape[0], V))
+    W = int(W)
+    if F * _lib.NGP_TEXTURE_MIN_SQUARE ** 2 > W * W:
+        raise RuntimeError("ngp_pl_b200.mesh.bake_texture: %d triangles need an atlas of size >= %d (%d squares of %d^2 "
+                           "texels), got %d" % (F, texture_size_for(F), F, _lib.NGP_TEXTURE_MIN_SQUARE, W))
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        ws_bytes = L.ngp_mesh_texture_workspace(V, F, W)
+        if ws_bytes == 0:
+            raise RuntimeError("ngp_pl_b200.mesh.bake_texture: %d vertices and %d triangles: both must be below 2^31"
+                               % (V, F))
+        _need(dev, ws_bytes + F * 36 + W * W * 3, "the atlas of %d triangles at size %d" % (F, W), "bake_texture")
+        ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+        uv = torch.empty(F, 3, 2, device=dev, dtype=torch.float32)
+        squares = torch.empty(F, 3, device=dev, dtype=torch.int32)
+        st = _st(dev)
+        cnt = (C.c_int64 * 2)()
+        _lib.check(L.ngp_mesh_texture_atlas(verts.data_ptr(), V, tris.data_ptr(), F, W, uv.data_ptr(), squares.data_ptr(),
+                                            cnt, ws.data_ptr(), ws_bytes, st), "ngp_mesh_texture_atlas")
+        n = int(cnt[1])
+        bake_bytes = L.ngp_mesh_texture_bake_workspace(int(samples))
+        _need(dev, n * 36 + W * W * 3 + bake_bytes, "%d band texels" % n, "bake_texture")
+        texel = torch.empty(n, device=dev, dtype=torch.int64)
+        tri = torch.empty(n, device=dev, dtype=torch.int32)
+        point = torch.empty(n, 3, device=dev, dtype=torch.float32)
+        normal = torch.empty(n, 3, device=dev, dtype=torch.float32)
+        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        _lib.check(L.ngp_mesh_texture_texels(verts.data_ptr(), ptr(nrm), V, tris.data_ptr(), F, W, uv.data_ptr(), n,
+                                             ptr(texel), ptr(tri), ptr(point), ptr(normal), ws.data_ptr(), ws_bytes, st),
+                   "ngp_mesh_texture_texels")
+        del ws
+        texture = torch.empty(W, W, 3, device=dev, dtype=torch.uint8)
+        bws = torch.empty(bake_bytes, device=dev, dtype=torch.uint8)
+        net, keep = _net_struct(model)
+        _lib.check(L.ngp_mesh_texture_bake(C.byref(net), W, n, ptr(texel), ptr(point), ptr(normal), r, int(samples),
+                                           texture.data_ptr(), bws.data_ptr(), bake_bytes, st), "ngp_mesh_texture_bake")
+        del bws
+    out = {"uv": uv, "squares": squares, "texture": texture}
+    if return_texels:
+        out.update(texel=texel, triangle=tri, point=point, normal=normal)
+    return out
+
+
 def _np(a):
     return a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+
+
+def _lines(fmt, a, chunk=1 << 18):
+    """fmt % row for every row of the 2-D array a, joined: one C-level format per chunk of rows, no per-line loop"""
+    parts = []
+    for i in range(0, a.shape[0], chunk):
+        b = a[i:i + chunk]
+        parts.append((fmt * b.shape[0]) % tuple(b.ravel().tolist()))
+    return "".join(parts)
+
+
+def write_obj(path, vertices, triangles, normals=None, uv=None, texture=None, png_mode="dynamic"):
+    """Wavefront OBJ: `v` per vertex (%.9g: fp32 round-trips), `vn` per vertex normal, with uv ((F, 3, 2) texel
+    coordinates as bake_texture returns them) 3F `vt` lines (uv / size, one per face corner, in face order), and faces
+    `f v/vt/vn` (1-based; v//vn, v/vt or v as the attributes present allow). size is texture's side, or the smallest
+    power of two >= 16 that holds the uv when no texture is given. With a texture ((W, W, 3) uint8, a device tensor) it
+    also writes <stem>.mtl, whose material maps <stem>.png, and that PNG, encoded on the device by images.encode_png
+    (png_mode "fixed" or "dynamic")."""
+    import os
+    v = _np(vertices).astype(np.float32).reshape(-1, 3)
+    f = _np(triangles).astype(np.int64).reshape(-1, 3)
+    F = f.shape[0]
+    stem = os.path.splitext(path)[0]
+    base = os.path.basename(stem)
+    head = "# ngp_pl_b200 mesh: %d vertices, %d triangles\n" % (v.shape[0], F)
+    png = None
+    if texture is not None:
+        from . import images
+        if not (isinstance(texture, torch.Tensor) and texture.dim() == 3 and texture.shape[0] == texture.shape[1]
+                and texture.shape[2] == 3 and texture.dtype == torch.uint8):
+            raise RuntimeError("ngp_pl_b200.mesh.write_obj: texture must be a (W, W, 3) uint8 tensor")
+        if uv is None:
+            raise RuntimeError("ngp_pl_b200.mesh.write_obj: a texture needs uv")
+        png = images.encode_png(texture.contiguous(), mode=png_mode)
+        head += "mtllib %s.mtl\nusemtl material0\n" % base
+    text = [head, _lines("v %.9g %.9g %.9g\n", v)]
+    if normals is not None:
+        text.append(_lines("vn %.9g %.9g %.9g\n", _np(normals).astype(np.float32).reshape(-1, 3)))
+    fi = f + 1
+    if uv is not None:
+        u = _np(uv).astype(np.float32).reshape(F * 3, 2)
+        W = texture.shape[0] if texture is not None else 16
+        while texture is None and W < u.max(initial=0):
+            W *= 2
+        text.append(_lines("vt %.9g %.9g\n", u / np.float32(W)))
+        vt = np.arange(1, 3 * F + 1, dtype=np.int64).reshape(F, 3)
+        if normals is not None:
+            text.append(_lines("f %d/%d/%d %d/%d/%d %d/%d/%d\n", np.stack([fi, vt, fi], 2).reshape(F, 9)))
+        else:
+            text.append(_lines("f %d/%d %d/%d %d/%d\n", np.stack([fi, vt], 2).reshape(F, 6)))
+    elif normals is not None:
+        text.append(_lines("f %d//%d %d//%d %d//%d\n", np.stack([fi, fi], 2).reshape(F, 6)))
+    else:
+        text.append(_lines("f %d %d %d\n", fi))
+    with open(path, "w", newline="\n") as fh:
+        fh.write("".join(text))
+    if png is not None:
+        with open(stem + ".mtl", "w", newline="\n") as fh:
+            fh.write("newmtl material0\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nillum 1\nmap_Kd %s.png\n" % base)
+        with open(stem + ".png", "wb") as fh:
+            fh.write(png)
 
 
 def write_ply(path, vertices, triangles, normals=None, colors=None):
