@@ -843,40 +843,61 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
 // level. Consecutive samples of a ray fall into the same cell at the coarse levels, so equal cells are
 // contiguous lane runs: their 16 corner contributions are summed with a segmented shuffle reduction and
 // only the head of each run issues the 8 vector reductions (fewer, and far less contended, L2 atomics).
+//
+// Level-major order: a work item is a chunk of SCATTER_THREADS consecutive samples x a group of SCATTER_GROUP
+// levels, and the tickets of the device counter hand out every chunk of one group before the next group. So
+// the reductions in flight hit one group's slice of the fp32 gradient (4 MB per hashed level at T = 2^19)
+// instead of the whole table (45.8 MB, about the size of the L2): a line stays in L2 across its reductions
+// instead of making a round trip to HBM for each. Group g holds levels g, g + G, g + 2G, ... (G groups), so
+// the small dense levels share their group with hashed ones rather than taking every SM's reductions alone.
+// An item reloads its chunk's positions; a larger group spends fewer reloads on a larger working set.
 // -------------------------------------------------------------------------------------------------
 #define SCATTER_THREADS 256
-__global__ void __launch_bounds__(SCATTER_THREADS)
+#define SCATTER_MIN_BLOCKS 5  // CTAs per SM: 40 warps (48 registers)
+#define SCATTER_GROUP 2       // levels per work item: 1 and 4 were slower (DESIGN.md section 9)
+__global__ void __launch_bounds__(SCATTER_THREADS, SCATTER_MIN_BLOCKS)
 k_grid_scatter_merged(const NgpNet net, const NgpSamples smp, const uint32_t* __restrict__ dfeat, const int64_t dfeat_stride,
-                      const float* __restrict__ loss_scale, float* __restrict__ grad_table) {
+                      const float* __restrict__ loss_scale, float* __restrict__ grad_table, int* __restrict__ sched) {
+    __shared__ int s_item[2];
     const int lane = threadIdx.x & 31;
     const int64_t n = bwd_count(smp);
-    const int64_t n_pad = (n + 31) & ~(int64_t)31;
     const int n_levels = net.meta.n_levels;
+    const int n_groups = (n_levels + SCATTER_GROUP - 1) / SCATTER_GROUP;
+    const int64_t n_chunks = (n + SCATTER_THREADS - 1) / SCATTER_THREADS;
+    const int64_t n_items = n_chunks * n_groups;
 
-    // the sample position is computed once and reused for all levels (dfeat is indexed by s, the position by the sample
-    // it stands for)
+    // an item's positions are computed once and reused for the levels of its group (dfeat is indexed by s, the position
+    // by the sample it stands for)
     bool valid;
     float u, v, w;
-    auto position = [&](int64_t s) {
+    int64_t s;
+    int group;
+    auto take = [&](int64_t item) {
+        group = (int)(item / n_chunks);
+        s = (item - group * n_chunks) * SCATTER_THREADS + threadIdx.x;
         valid = s < n;
         const SampleIn sm = load_sample(smp, (valid && smp.live_idx) ? (int64_t)__ldg(smp.live_idx + s) : s, valid);
         to_unit(net, sm, u, v, w);
     };
-    // this thread's first sample (the count, the live list and the positions were written two or more kernels earlier) is
-    // loaded before waiting on the MLP backward, whose feature gradients are the first thing read after it
-    int64_t s = blockIdx.x * (int64_t)SCATTER_THREADS + threadIdx.x;
-    position(s);
+    // the first item's positions (the count, the live list and the positions were written two or more kernels earlier)
+    // are loaded before waiting on the MLP backward, whose feature gradients are the first thing read after it
+    if (threadIdx.x == 0) s_item[0] = sched ? atomicAdd(&sched[0], 1) : (int)blockIdx.x;
+    __syncthreads();
+    int64_t item = s_item[0];
+    if (item < n_items) take(item);
     pdl_wait();
     pdl_trigger();
     const float inv_scale = loss_scale ? 1.0f / *loss_scale : 1.0f;
-    for (; s < n_pad; s += (int64_t)gridDim.x * SCATTER_THREADS, position(s)) {
+    for (int it = 0; item < n_items; ++it) {
+        // the next ticket travels while this item is scattered
+        if (threadIdx.x == 0) s_item[(it + 1) & 1] = sched ? atomicAdd(&sched[0], 1) : (int)(item + gridDim.x);
         const unsigned vmask = __ballot_sync(0xffffffffu, valid);
         // the per-level feature gradient is the one load on the critical path of a level: fetch the NEXT level's while
         // this level's shuffles and reductions run
-        uint32_t d_next = valid ? __ldg(dfeat + s) : 0u;
-        for (int level = 0; level < n_levels; ++level) {
+        uint32_t d_next = valid ? __ldg(dfeat + (int64_t)group * dfeat_stride + s) : 0u;
+        for (int level = group; level < n_levels; level += n_groups) {
             const uint32_t d_cur = d_next;
-            if (valid && level + 1 < n_levels) d_next = __ldg(dfeat + (int64_t)(level + 1) * dfeat_stride + s);
+            if (valid && level + n_groups < n_levels) d_next = __ldg(dfeat + (int64_t)(level + n_groups) * dfeat_stride + s);
             const uint32_t res = net.meta.res[level];
             const uint32_t off = net.meta.offset[level];
             const uint32_t entries = net.meta.offset[level + 1] - off;
@@ -930,7 +951,11 @@ k_grid_scatter_merged(const NgpNet net, const NgpSamples smp, const uint32_t* __
                 grid_scatter_cell_paired(lvl, idx, acc);  // 16-byte reductions for aligned x-corner pairs, 8-byte otherwise
             }
         }
+        __syncthreads();
+        item = s_item[(it + 1) & 1];
+        if (item < n_items) take(item);
     }
+    sched_finish(sched);
 }
 
 // workspace of ngp_net_backward: the feature gradients, one half2 per (level, sample): 64 B per sample
@@ -978,11 +1003,14 @@ extern "C" int ngp_net_backward_scatter(const NgpNet* net, const NgpSamples* smp
     if (!grad_enc || (smp->live_idx && !smp->n_live_dev)) return NGP_EINVAL;
     if (smp->n == 0) return 0;
     const int64_t n_mtiles = (smp->n + 15) / 16;
-    int64_t gx = (smp->n + SCATTER_THREADS - 1) / SCATTER_THREADS;
-    const int64_t cap = (int64_t)ngp_sm_count() * 8;
+    // persistent: as many CTAs as are resident at once, at most one per item of the capacity
+    const int n_groups = (net->meta.n_levels + SCATTER_GROUP - 1) / SCATTER_GROUP;
+    int64_t gx = (smp->n + SCATTER_THREADS - 1) / SCATTER_THREADS * n_groups;
+    const int64_t cap = (int64_t)ngp_sm_count() * SCATTER_MIN_BLOCKS;
     if (gx > cap) gx = cap;
     NGP_CUDA(ngp_launch_pdl(k_grid_scatter_merged, (unsigned)gx, SCATTER_THREADS, 0, (cudaStream_t)stream, *net, *smp,
-                            (const uint32_t*)workspace, n_mtiles * 16, loss_scale, grad_enc + NGP_DENSITY_MLP_PARAMS));
+                            (const uint32_t*)workspace, n_mtiles * 16, loss_scale, grad_enc + NGP_DENSITY_MLP_PARAMS,
+                            sched_slot((cudaStream_t)stream)));
     NGP_CHECK_LAUNCH();
     NGP_TRACE(7, (cudaStream_t)stream);
     return 0;
