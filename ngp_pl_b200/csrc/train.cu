@@ -494,8 +494,11 @@ __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __re
                        float beta1, float beta2, float eps, float grad_mul) {
     const AdamConsts c = adam_consts(lr_dev, step_dev, beta1, beta2, eps, grad_mul);
     const int64_t n4 = n >> 2;
-    // fp32 params, moments and the consumed gradients stream through L2 (evict first); the fp16 working copy the
-    // forward gathers from is kept (evict last); the zeroed gradients (next step's reduction target) stay normal
+    // fp32 params and moments stream through L2 (evict first); the fp16 working copy the forward gathers from is kept
+    // (evict last). The gradients are loaded and cleared with the normal policy: the clear is a 16-byte store only where
+    // g != 0, and it should find its line still in L2. Loaded evict-first, the kernel ran 12 % (config 2) to 15 %
+    // (config 5) slower, most likely because the line was gone by then and the clear reached HBM as a partial sector
+    // (DESIGN.md §9).
     const uint64_t stream_pol = l2_policy_evict_first(), keep_pol = l2_policy_evict_last();
     // two 64-byte groups per thread and trip: all eight 128-bit loads are issued before the first use, so the stream keeps
     // ~15 MB in flight even when the next step's march shares the SMs' issue slots
@@ -523,7 +526,7 @@ __global__ void k_adam(float* __restrict__ p, float* __restrict__ g, float* __re
         }
 #pragma unroll
         for (int u = 0; u < 2; ++u)
-            if (u == 0 || two) gv[u] = ld_f4_hint(reinterpret_cast<const float4*>(g) + (u ? i1 : i0), stream_pol);
+            if (u == 0 || two) gv[u] = reinterpret_cast<const float4*>(g)[u ? i1 : i0];
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
             if (u == 1 && !two) break;
