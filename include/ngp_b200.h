@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 11
+#define NGP_ABI_VERSION 12
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -804,6 +804,68 @@ size_t ngp_mesh_texture_bake_workspace(int samples);
 int ngp_mesh_texture_bake(const NgpNet* net, int size, int64_t n_texels, const int64_t* texel, const float* point,
                           const float* normal, float offset, int samples, uint8_t* texture, void* workspace,
                           size_t workspace_bytes, void* stream);
+
+/* Point-cloud export: a coloured point cloud with normals from the training views' rendered depth. numpy float64
+ * restatement: oracle/points_ref.py. Stages (ngp_pl_b200/points.py runs them in this order):
+ *   1. Rays, no RNG: N = n_views * n_pix global pixels, R = min(num_rays, N). Ray k takes q_k = (k g) mod N, the
+ *      product exact (128-bit), with g the smallest integer >= round(0.6180339887 N) (half up, exact integers) coprime
+ *      to N, found on the host; k -> q_k is then a bijection of 0..N-1, so the first R rays have no duplicate. View
+ *      q div n_pix, pixel q mod n_pix; the rays are ngp_gen_rays' on that (img_idx, pix_idx) list.
+ *   2. Render: ngp_render_infer_frame with bg = 0 (opacity, depth and rgb as it writes them), in batches of a fixed
+ *      ray count: its per-round quota follows the batch's alive count, so the batch size is part of the result.
+ *   3. Back-projection, fp32: t = __fdiv_rn(depth, opacity), p = fmaf(d, t, o) per axis, colour = rint(255 min(
+ *      __fdiv_rn(rgb, opacity), 1)), view = d / sqrt((dx dx + dy dy) + dz dz) (each operation rounded). A ray is kept
+ *      iff opacity >= min_opacity (in (0, 1]), p is finite and p lies in the closed box bounds[0..2] .. bounds[3..5].
+ *      Kept points stay in ray order.
+ *   4. Voxel downsampling on a cluster grid (rule 1 of the mesh simplification: the same cell and key): one point per
+ *      occupied cell, in ascending key. Position = the double mean of the members rounded to fp32, colour =
+ *      floor(mean + 1/2) from integer sums, view = the normalised double sum of the members' views (0 when it is 0).
+ *   5. k nearest neighbours, k in 1..min(NGP_POINTS_MAX_K, n - 1): for every point the k smallest pairs (d^2, j) over
+ *      the other points j (duplicates included), d^2 = (ex ex + ey ey) + ez ez in double of e = p_j - p_i from the fp32
+ *      coordinates, ordered by d^2 and then j. Exact: a uniform grid (at most NGP_POINTS_KNN_MAX_CELLS cells) searched
+ *      ring by ring until no unvisited cell can hold a closer point.
+ *   6. Statistical outlier removal: d_i = the mean of sqrt(d^2) over the k neighbours; mu and sigma (population) of the
+ *      d_i in double, fixed-order reductions; a point is kept iff d_i <= mu + std_ratio sigma, in order.
+ *   7. Normals: the covariance sum (x - m)(x - m)^T over the point and its k neighbours about their mean m, in double;
+ *      the eigenvector of the smallest eigenvalue (the first on a tie) from NGP_SIMPLIFY_JACOBI_SWEEPS cyclic Jacobi
+ *      sweeps, negated when n . view > 0, rounded to fp32; (0, 0, 0) when the covariance is 0.
+ * No float atomics: two calls are bitwise equal.
+ *
+ * ngp_points_rays: rays k0 .. k0 + n - 1 (k0 + n <= N, 1 <= g < N or g = 1 for N = 1): img_idx, pix_idx (n) int64 and
+ * rays_o, rays_d (n, 3) fp32 from poses (n_views, 3, 4) and directions (n_pix, 3).
+ * ngp_points_backproject: stage 3 over n rays; the kept points go to points (3 fp32), colors (3 uint8) and views
+ * (3 fp32) from their first row, and their number to the host int64 *count (one read-back: the call synchronises the
+ * stream). bounds is host memory.
+ * ngp_points_voxel: stage 4 into outputs of capacity n; out_keys (int64 cluster keys) and out_counts (int32 members) may
+ * be NULL; the number of cells to *count (a read-back).
+ * ngp_points_knn: stage 5; idx (n, k) int32 and dist2 (n, k) double. One read-back (the box). NGP_EINVAL also for a
+ * coordinate that is not finite.
+ * ngp_points_outliers: stage 6 over dist2 (n, k) as ngp_points_knn writes it (n >= 2); the kept points to the out arrays
+ * (capacity n), their input indices to kept (may be NULL), {mu, sigma, threshold} to the host double stats[3] (may be
+ * NULL) and their number to *count (a read-back).
+ * ngp_points_normals: stage 7 with idx (n, k) from ngp_points_knn (k may be 0: every normal is then 0); no read-back.
+ * ngp_points_workspace(n) covers every call above for up to n points or rays (0 for n outside [0, 2^31)). All calls
+ * return NGP_EINVAL for sizes out of range, a NULL pointer that is needed or a short workspace. */
+#define NGP_POINTS_MAX_K 64
+#define NGP_POINTS_KNN_MAX_CELLS (1 << 22)
+size_t ngp_points_workspace(int64_t n);
+int ngp_points_rays(int64_t n_views, int64_t n_pix, int64_t g, int64_t k0, int n, const float* poses,
+                    const float* directions, int64_t* img_idx, int64_t* pix_idx, float* rays_o, float* rays_d, void* stream);
+int ngp_points_backproject(const float* rays_o, const float* rays_d, const float* opacity, const float* depth,
+                           const float* rgb, int64_t n, float min_opacity, const float* bounds, float* points,
+                           uint8_t* colors, float* views, int64_t* count, void* workspace, size_t workspace_bytes,
+                           void* stream);
+int ngp_points_voxel(const float* points, const uint8_t* colors, const float* views, int64_t n, const NgpClusterGrid* grid,
+                     float* out_points, uint8_t* out_colors, float* out_views, int64_t* out_keys, int32_t* out_counts,
+                     int64_t* count, void* workspace, size_t workspace_bytes, void* stream);
+int ngp_points_knn(const float* points, int64_t n, int k, int32_t* idx, double* dist2, void* workspace,
+                   size_t workspace_bytes, void* stream);
+int ngp_points_outliers(const float* points, const uint8_t* colors, const float* views, int64_t n, int k,
+                        const double* dist2, double std_ratio, float* out_points, uint8_t* out_colors, float* out_views,
+                        int32_t* kept, double* stats, int64_t* count, void* workspace, size_t workspace_bytes,
+                        void* stream);
+int ngp_points_normals(const float* points, const float* views, int64_t n, int k, const int32_t* idx, float* normals,
+                       void* stream);
 
 /* ----------------------------------------------------------------------------------------------
  * Test-view images of the validation pass (reference train.py:215-221): `{idx:03d}.png` holds (rgb_pred*255).astype(np.uint8)

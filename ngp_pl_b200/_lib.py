@@ -9,7 +9,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 11  #NGP_ABI_VERSION in include/ngp_b200.h
+ABI_VERSION = 12  #NGP_ABI_VERSION in include/ngp_b200.h
 
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
@@ -25,6 +25,8 @@ NGP_TEXTURE_MIN_SQUARE = 4
 NGP_TEXTURE_MARGIN = 1
 NGP_TEXTURE_MAX_SAMPLES = 256
 NGP_TEXTURE_CHUNK_SAMPLES = 1 << 22
+NGP_POINTS_MAX_K = 64
+NGP_POINTS_KNN_MAX_CELLS = 1 << 22
 NGP_VIEW_IMAGES_WORKSPACE = 4096
 NGP_PNG_FIXED = 0
 NGP_PNG_DYNAMIC = 1
@@ -238,6 +240,13 @@ SIGNATURES = {
     "ngp_mesh_texture_texels": (_i, [_P, _P, _i64, _P, _i64, _i, _P, _i64, _P, _P, _P, _P, _P, _sz, _P]),
     "ngp_mesh_texture_bake_workspace": (_sz, [_i]),
     "ngp_mesh_texture_bake": (_i, [C.POINTER(NgpNet), _i, _i64, _P, _P, _P, _f, _i, _P, _P, _sz, _P]),
+    "ngp_points_workspace": (_sz, [_i64]),
+    "ngp_points_rays": (_i, [_i64, _i64, _i64, _i64, _i, _P, _P, _P, _P, _P, _P, _P]),
+    "ngp_points_backproject": (_i, [_P, _P, _P, _P, _P, _i64, _f, _P, _P, _P, _P, _P, _P, _sz, _P]),
+    "ngp_points_voxel": (_i, [_P, _P, _P, _i64, C.POINTER(NgpClusterGrid), _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
+    "ngp_points_knn": (_i, [_P, _i64, _i, _P, _P, _P, _sz, _P]),
+    "ngp_points_outliers": (_i, [_P, _P, _P, _i64, _i, _P, C.c_double, _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
+    "ngp_points_normals": (_i, [_P, _P, _i64, _i, _P, _P, _P]),
     "ngp_view_images": (_i, [_P, _P, _i, _i, _P, _P, _P, _sz, _P]),
     "ngp_png_workspace": (_sz, [_i, _i]),
     "ngp_png_capacity": (_sz, [_i, _i]),

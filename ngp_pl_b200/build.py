@@ -16,9 +16,10 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libngp_b200.so")
 
 SOURCES = ["vren_ops.cu", "network.cu", "train.cu", "infer.cu", "modules.cu", "metrics.cu", "mesh.cu", "lpips.cu", "stage.cu", "images.cu", "jpeg.cu",
-           "texture.cu"]
-# texture.cu's double arithmetic must round operation by operation as its numpy restatement (oracle/mesh_texture.py) does
-SOURCE_FLAGS = {"texture.cu": ["-fmad=false"]}
+           "texture.cu", "points.cu"]
+# texture.cu's and points.cu's double arithmetic must round operation by operation as their numpy restatements
+# (oracle/mesh_texture.py, oracle/points_ref.py) do
+SOURCE_FLAGS = {"texture.cu": ["-fmad=false"], "points.cu": ["-fmad=false"]}
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
