@@ -201,7 +201,9 @@ int ngp_net_backward_scatter(const NgpNet* net, const NgpSamples* smp, const flo
  *   ngp_mlp_rgb_forward  : tcnn.Network 32->64->64->3 on x fp16 (n,32) -> fp16 (n,3)
  *   ngp_mlp_rgb_backward : dL/dout fp32 (n,3) -> dL/dx fp32 (n,32) (optional) and grad_rgb (+=, fp32 7168)
  *   ngp_enc_backward     : tcnn.NetworkWithInputEncoding backward from dL/dh fp32 (n,16); forward is
- *                          ngp_net_forward(want_rgb=0, h_out, feat_save); workspace as ngp_net_backward */
+ *                          ngp_net_forward(want_rgb=0, h_out, feat_save); workspace as ngp_net_backward
+ * Alignment (NGP_EINVAL otherwise, before any device work): x_half 4 B, dL_dx and dL_dh 8 B, out_half and
+ * feat_save 16 B. */
 int ngp_sh_encode(const float* u01, int64_t n, uint16_t* out_half, void* stream);
 int ngp_mlp_rgb_forward(const uint16_t* rgb_params_h, const uint16_t* x_half, int64_t n, int rgb_act, uint16_t* out_half3,
                         void* stream);

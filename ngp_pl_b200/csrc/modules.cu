@@ -259,7 +259,10 @@ k_mlp_rgb_bwd(const __half* __restrict__ wr, const __half* __restrict__ X, const
 
 extern "C" int ngp_mlp_rgb_backward(const uint16_t* rgb_params_h, const uint16_t* x_half, const float* dL_dout3, int64_t n,
                                     int rgb_act, const float* loss_scale, float* dL_dx, float* grad_rgb, void* stream) {
-    if (n < 0 || !rgb_params_h || !grad_rgb || (n > 0 && (!x_half || !dL_dout3)) || (((uintptr_t)dL_dx) & 7)) return NGP_EINVAL;
+    // x_half is read as uint32 (load_rows32), dL_dx written as float2
+    if (n < 0 || !rgb_params_h || !grad_rgb || (n > 0 && (!x_half || !dL_dout3)) || (((uintptr_t)x_half) & 3) ||
+        (((uintptr_t)dL_dx) & 7))
+        return NGP_EINVAL;
     if (n == 0) return 0;
     NGP_CUDA(ngp_smem_opt_in<k_mlp_rgb_bwd>((int)sizeof(RgbBwdSmem)));
     const int64_t n_blks = ((n + 15) / 16 + MOD_WARPS - 1) / MOD_WARPS;
@@ -375,8 +378,11 @@ k_enc_bwd(const __half* __restrict__ wd, const uint4* __restrict__ feat_save, co
 extern "C" int ngp_enc_backward(const NgpNet* net, const NgpSamples* smp, const float* dL_dh, const void* feat_save,
                                 const float* loss_scale, float* grad_enc, void* workspace, size_t workspace_bytes, void* stream) {
     if (!net || !smp || smp->n < 0 || !grad_enc) return NGP_EINVAL;
+    if (net->meta.n_levels < 1 || net->meta.n_levels > NGP_MAX_LEVELS) return NGP_EINVAL;
     if (smp->n == 0) return 0;
     if (!dL_dh || !feat_save || !workspace || workspace_bytes < ngp_net_backward_workspace(smp->n)) return NGP_EINVAL;
+    // dL_dh is read as float2, feat_save as uint4
+    if ((((uintptr_t)dL_dh) & 7) || (((uintptr_t)feat_save) & 15)) return NGP_EINVAL;
     NGP_CUDA(ngp_smem_opt_in<k_enc_bwd>((int)sizeof(EncBwdSmem)));
     const int64_t n_mtiles = (smp->n + 15) / 16;
     const int64_t n_blks = (n_mtiles + MOD_WARPS - 1) / MOD_WARPS;

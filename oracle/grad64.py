@@ -23,6 +23,10 @@ A row whose ReLU masks are not determined by those intervals is flagged in `ambi
 reference may take different branches and no rounding bound applies. `ambiguous_own` flags the subset where the
 pre-activation's own accumulation error alone (|z| <= 2^-20 sum|terms|) leaves the mask open.
 
+rgb_backward() and density_backward() are the two halves of that chain on their own, as the stand-alone module kernels
+run them: k_mlp_rgb_bwd from an fp16 input matrix to dL/dx in fp32 (no fp16 rounding), k_enc_bwd from a scaled fp16
+dL/dh to the feature gradients. mlp_backward() composes them with the one rounding k_ngp_bwd3 adds in between.
+
 mlp_forward() is that forward on its own, as intervals (with carry=True every bound is followed to the outputs);
 grid_encode(), sigma(), sh_encode(), ray_positions() and to_unit() restate the rest of k_ngp_fwd / k_sh_encode: the
 hash-grid features, sigma = expf(h0), the stand-alone SH encoding and the sample positions, each with its derived bound
@@ -37,6 +41,7 @@ import torch
 ULP16 = 2.0 ** -10   # one fp16 ulp, relative (normal range): a rounding (2^-11) plus a flipped last bit
 SUB16 = 2.0 ** -24   # smallest fp16 subnormal: absolute floor of a rounding
 ACC32 = 2.0 ** -20   # fp32 tensor-core accumulation of <= 64 fp16 products, relative to sum |terms|
+ACC32_OUT = 2.0 ** -24  # one fp32 rounding of a stored result, relative
 SH_ERR = 2.0 ** -19  # absolute error of the kernel's fp32 SH-4 of a normalised direction (|SH| <= 3, degree <= 3)
 SIG_ERR = 2.0 ** -19  # absolute error of the kernel's fp32 sigmoid 1 / (1 + __expf(-x))
 M32 = 0xFFFFFFFF
@@ -182,30 +187,27 @@ def mlp_forward(feat, sh, enc_mlp, rgb_params, rgb_act=1, carry=False, d_feat=No
     return f
 
 
-def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1):
-    """feat (n, 32) fp16 features, sh (n, 16) float64 SH-4 (unrounded), enc_mlp (>= 3072) / rgb_params (7168) fp16 weights,
-    up_sig (n), up_rgb (n, 3) fp32 upstream gradients, scale the power-of-two loss scale (a number).
-    Returns a dict: dfeat (n, 32, scaled by `scale`, like the kernel's workspace), dfeat_err, dfeat_abs, ambiguous (n) bool,
-    dW {name: (value, A, err)} for W3r, W2r, W1r, W2d, W1d (unscaled), and the forward activations."""
+def rgb_backward(rin, d_rin, rgb_params, up_rgb, scale, rgb_act=1):
+    """k_mlp_rgb_bwd's chain from fp16 inputs rin (n, 32) the kernel may hold differently by up to d_rin (0 when they are
+    the kernel's own input), fp32 upstream gradients up_rgb (n, 3) and the power-of-two loss scale:
+      dout = fp16(up o (1 - o) scale),  dr2 = fp16([r2 > 0] dout W3r),  dr1 = fp16([r1 > 0] dr2 W2r)
+      dX   = (dr1 W1r) / scale in fp32: all 32 columns, no fp16 rounding
+    Returns a dict: dX (n, 32, unscaled), dX_err (its bound: the operand errors and the fp32 accumulation of dr1 W1r,
+    plus one fp32 rounding), dX_abs; dout / dr2 / dr1 with _err / _abs (scaled); dW {W3r, W2r, W1r: (value, A, err)}
+    (unscaled); ambiguous / ambiguous_own (n) bool; the forward dict `fwd` (rgb_forward's)."""
     dt = torch.float64
-    feat = feat.to(dt)
-    n = feat.shape[0]
-    Wd, Wr = enc_mlp.to(dt), rgb_params.to(dt)
-    W1d, W2d = Wd[:2048].view(64, 32), Wd[2048:3072].view(16, 64)
+    Wr = rgb_params.to(dt)
     W1r, W2r, W3r = Wr[:2048].view(64, 32), Wr[2048:6144].view(64, 64), Wr[6144:7168].view(16, 64)
-    up_sig, up_rgb = up_sig.to(dt), up_rgb.to(dt)
-
-    # ---- forward recompute with the kernel's rounding points, as intervals ----
-    f = mlp_forward(feat, sh, enc_mlp, rgb_params, rgb_act)
-    hid, d_hid, h, d_h, rin, d_rin = f["hid"], f["d_hid"], f["h"], f["d_h"], f["rin"], f["d_rin"]
-    r1, d_r1, r2, d_r2, yo = f["r1"], f["d_r1"], f["r2"], f["d_r2"], f["yo"]
+    up_rgb = up_rgb.to(dt)
+    f = rgb_forward(rin, d_rin, rgb_params, rgb_act)
+    rin, d_rin, r1, d_r1, r2, d_r2, yo = f["rin"], f["d_rin"], f["r1"], f["d_r1"], f["r2"], f["d_r2"], f["yo"]
+    n = rin.shape[0]
     if rgb_act == 1:
-        o, s, ds = f["out"], f["s"], f["d_s"]
+        s, ds = f["s"], f["d_s"]
     else:
         s, ds = torch.ones_like(yo), torch.zeros_like(yo)
 
-    # ---- out-gradient chain ----
-    dout = torch.zeros(n, 16, dtype=dt, device=feat.device)
+    dout = torch.zeros(n, 16, dtype=dt, device=rin.device)
     dout_abs, dout_err = torch.zeros_like(dout), torch.zeros_like(dout)
     v = up_rgb * s * scale
     dout[:, :3] = f16(v)
@@ -213,6 +215,72 @@ def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1
     dout_err[:, :3] = _round_err(ACC32 * v.abs() + up_rgb.abs() * ds * scale, v.abs())
     dr2, dr2_err, dr2_abs = _chain(dout, dout_err, dout_abs, W3r, (r2 > 0).to(dt))
     dr1, dr1_err, dr1_abs = _chain(dr2, dr2_err, dr2_abs, W2r, (r1 > 0).to(dt))
+    W1a = W1r.abs()
+    y, a = dr1 @ W1r, dr1_abs @ W1a
+    e = dr1_err @ W1a + ACC32 * a
+    # the fp32 accumulator times 1 / scale (a power of two: exact) is stored once, rounded to fp32; 2^-149 is its
+    # subnormal floor
+    dX_err = (e + ACC32_OUT * (y.abs() + e)) / scale + 2.0 ** -149
+    dW = {
+        "W3r": _wgrad(dout, dout_err, dout_abs, r2, d_r2, scale),
+        "W2r": _wgrad(dr2, dr2_err, dr2_abs, r1, d_r1, scale),
+        "W1r": _wgrad(dr1, dr1_err, dr1_abs, rin, d_rin, scale),
+    }
+    return dict(dX=y / scale, dX_err=dX_err, dX_abs=a / scale, dout=dout, dout_err=dout_err, dout_abs=dout_abs,
+                dr2=dr2, dr2_err=dr2_err, dr2_abs=dr2_abs, dr1=dr1, dr1_err=dr1_err, dr1_abs=dr1_abs, dW=dW,
+                ambiguous=f["ambiguous"], ambiguous_own=f["ambiguous_own"], fwd=f)
+
+
+def scaled_dh(dL_dh, scale):
+    """k_enc_bwd's out-gradient: dh = fp16(dL_dh scale), a single rounding of an fp32 product (no accumulation).
+    -> (value, bound, absolute value), float64 (n, 16), scaled"""
+    v = dL_dh.double() * scale
+    return f16(v), _round_err(torch.zeros_like(v), v.abs()), v.abs()
+
+
+def density_backward(feat, enc_mlp, dh, dh_err, dh_abs, scale):
+    """k_enc_bwd's chain (and the density half of k_ngp_bwd3's) from the fp16 features feat (n, 32) and the scaled fp16
+    out-gradient dh (n, 16), which the kernel may hold differently by up to dh_err (dh_abs: its absolute-value chain):
+      dhid = fp16([hid > 0] dh W2d),  dfeat = fp16(dhid W1d)
+    Returns a dict: dhid / dfeat (scaled, like the kernel's workspace) with _err / _abs; dW {W2d, W1d: (value, A, err)}
+    (unscaled); hid, d_hid; ambiguous / ambiguous_own (n) bool: rows whose hidden-layer ReLU mask is open."""
+    dt = torch.float64
+    feat = feat.to(dt)
+    Wd = enc_mlp.to(dt)
+    W1d, W2d = Wd[:2048].view(64, 32), Wd[2048:3072].view(16, 64)
+    hid, d_hid, amb = _fwd(feat, torch.zeros_like(feat), W1d, True)
+    dhid, dhid_err, dhid_abs = _chain(dh, dh_err, dh_abs, W2d, (hid > 0).to(dt))
+    dfeat, dfeat_err, dfeat_abs = _chain(dhid, dhid_err, dhid_abs, W1d, None)
+    dW = {
+        "W2d": _wgrad(dh, dh_err, dh_abs, hid, d_hid, scale),
+        "W1d": _wgrad(dhid, dhid_err, dhid_abs, feat, torch.zeros_like(feat), scale),
+    }
+    return dict(dhid=dhid, dhid_err=dhid_err, dhid_abs=dhid_abs, dfeat=dfeat, dfeat_err=dfeat_err, dfeat_abs=dfeat_abs,
+                dW=dW, hid=hid, d_hid=d_hid, ambiguous=amb[0], ambiguous_own=amb[1])
+
+
+def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1):
+    """feat (n, 32) fp16 features, sh (n, 16) float64 SH-4 (unrounded), enc_mlp (>= 3072) / rgb_params (7168) fp16 weights,
+    up_sig (n), up_rgb (n, 3) fp32 upstream gradients, scale the power-of-two loss scale (a number).
+    Returns a dict: dfeat (n, 32, scaled by `scale`, like the kernel's workspace), dfeat_err, dfeat_abs, ambiguous (n) bool,
+    dW {name: (value, A, err)} for W3r, W2r, W1r, W2d, W1d (unscaled), and the forward activations.
+    It is rgb_backward, then the sum k_ngp_bwd3 rounds once: dh = fp16(dr1 W1r[:, 16:] + up_sig exp(h0) scale in
+    column 0), then density_backward."""
+    dt = torch.float64
+    feat = feat.to(dt)
+    Wr = rgb_params.to(dt)
+    W1r = Wr[:2048].view(64, 32)
+    up_sig = up_sig.to(dt)
+
+    # ---- forward recompute with the kernel's rounding points, as intervals ----
+    f = mlp_forward(feat, sh, enc_mlp, rgb_params, rgb_act)
+    hid, h, d_h, rin, r1, r2, yo = f["hid"], f["h"], f["d_h"], f["rin"], f["r1"], f["r2"], f["yo"]
+    if rgb_act == 1:
+        o = f["out"]
+
+    # ---- out-gradient chain ----
+    rb = rgb_backward(rin, f["d_rin"], rgb_params, up_rgb, scale, rgb_act)
+    dout, dr2, dr1, dr1_err, dr1_abs = rb["dout"], rb["dr2"], rb["dr1"], rb["dr1_err"], rb["dr1_abs"]
     Wh = W1r[:, 16:]
     y, a, e = dr1 @ Wh, dr1_abs @ Wh.abs(), dr1_err @ Wh.abs()
     # density branch d sigma / d h0 = exp(clamp(h0, -15, 15)), h0 possibly off by d_h[:, 0]
@@ -224,20 +292,14 @@ def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1
     a[:, 0] += t.abs()
     e[:, 0] += dt0
     dh, dh_err, dh_abs = f16(y), _round_err(e + ACC32 * a, a), a
-    dhid, dhid_err, dhid_abs = _chain(dh, dh_err, dh_abs, W2d, (hid > 0).to(dt))
-    dfeat, dfeat_err, dfeat_abs = _chain(dhid, dhid_err, dhid_abs, W1d, None)
+    db = density_backward(feat, enc_mlp, dh, dh_err, dh_abs, scale)
 
-    dW = {
-        "W3r": _wgrad(dout, dout_err, dout_abs, r2, d_r2, scale),
-        "W2r": _wgrad(dr2, dr2_err, dr2_abs, r1, d_r1, scale),
-        "W1r": _wgrad(dr1, dr1_err, dr1_abs, rin, d_rin, scale),
-        "W2d": _wgrad(dh, dh_err, dh_abs, hid, d_hid, scale),
-        "W1d": _wgrad(dhid, dhid_err, dhid_abs, feat, torch.zeros_like(feat), scale),
-    }
-    return dict(dfeat=dfeat, dfeat_err=dfeat_err, dfeat_abs=dfeat_abs, dW=dW,
+    dW = dict(rb["dW"])
+    dW.update(db["dW"])
+    return dict(dfeat=db["dfeat"], dfeat_err=db["dfeat_err"], dfeat_abs=db["dfeat_abs"], dW=dW,
                 ambiguous=f["ambiguous"], ambiguous_own=f["ambiguous_own"],
                 hid=hid, h=h, rin=rin, r1=r1, r2=r2, o=o if rgb_act == 1 else yo,
-                chain=[dout, dr2, dr1, dh, dhid, dfeat])
+                chain=[dout, dr2, dr1, dh, db["dhid"], db["dfeat"]])
 
 
 # layout of the five weight gradients in the flat parameter-gradient vectors: (vector, offset, shape)

@@ -362,17 +362,25 @@ def test_capacity_below_the_marched_total_guarded(path):
     run_fused(tr, o, d, gt, noise)
     marched = tr.n_samples.long().clone()
     total = int(marched.sum())
-    cap = int(0.6 * total)
-    tr.cfg.max_total_samples = cap
-    tr.capacity = cap
-    guarded = fill_guard(tr, cap)
-    capacity_step(tr, o, d, gt, noise, cap, marched)
-    label = "guarded %s cap=%d of %d" % (path, cap, total)
-    check_guard(guarded, cap, label)
-    _, off, cnt = check_step(tr, gt, bgc, cap, label)
-    full = tr.n_samples.long()
-    past = (cnt == 0) & (full > 0)
-    straddle = (cnt > 0) & (cnt < full)
+    # the rays arrive in a different order every run, and a capacity that lands exactly on the end of a ray's segment
+    # (about 1 run in 40 here) leaves no ray straddling it: then the step is checked as it is and taken again one sample
+    # lower, until some ray straddles the capacity
+    for attempt in range(4):
+        cap = int(0.6 * total) - attempt
+        tr.cfg.max_total_samples = cap
+        tr.capacity = cap
+        guarded = fill_guard(tr, cap)
+        capacity_step(tr, o, d, gt, noise, cap, marched)
+        label = "guarded %s cap=%d of %d" % (path, cap, total)
+        check_guard(guarded, cap, label)
+        _, off, cnt = check_step(tr, gt, bgc, cap, label)
+        full = tr.n_samples.long()
+        past = (cnt == 0) & (full > 0)
+        straddle = (cnt > 0) & (cnt < full)
+        if straddle.sum() >= 1:
+            break
+        # no straddling ray: the capacity is exactly the end of one ray's segment
+        assert bool(((off + cnt == cap) & (cnt == full) & (cnt > 0)).any()), label
     assert past.sum() > 10 and straddle.sum() >= 1, label
     # a ray past the capacity renders the background alone
     assert (tr.opacity[past] == 0).all() and (tr.rgb[past] == torch.tensor(bgc, device="cuda")).all()

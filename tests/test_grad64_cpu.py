@@ -3,9 +3,12 @@ silently agree with a wrong kernel (tests/test_backward_fp64_gpu.py compares the
   * its network backward against fp32 autograd of oracle.torch_ngp_forward (rgb_act 0 and 1);
   * its table scatter against float64 autograd of oracle.torch_grid_encode (dense, hashed and wrapping corners);
   * its feat_save decoder against a plain encoder of the documented fragment layout;
+  * its two halves, rgb_backward and density_backward (the stand-alone module kernels' chains), against float64 autograd
+    at the kernels' rounding points, and their bounds around an fp32 restatement of the kernels;
   * mlp_backward against its own stored outputs (tests/golden/grad64_mlp_backward.npz), so that a change to the forward
     it shares with mlp_forward shows.
 """
+import math
 import os
 
 import numpy as np
@@ -263,3 +266,120 @@ def test_sh_encode_and_ray_positions_restatements():
             ties = [c for c, e in zip(cands, dist) if e == best]
             want = ties[0] if len(ties) == 1 else [c for c in ties if not (c.view(np.int32) & 1)][0]
             assert x[i, k] == want, (i, k, float(x[i, k]), float(want))
+
+
+def _ste16(v):
+    """fp16 rounding in the forward value, identity in the gradient (autograd then differentiates the unrounded chain at
+    the kernel's rounded activations)"""
+    return v + (grad64.f16(v.detach()) - v.detach())
+
+
+@pytest.mark.parametrize("rgb_act", [1, 0])
+def test_rgb_backward_vs_float64_autograd_and_fp32(rgb_act):
+    """rgb_backward (k_mlp_rgb_bwd's chain from an external fp16 input) against float64 autograd of the rgb net at the
+    kernel's rounding points, and its bounds around an fp32 restatement of the kernel"""
+    _, rgb = _params(0, 41)
+    g = torch.Generator().manual_seed(42)
+    n = 300
+    rin = (torch.rand(n, 32, generator=g) * 2 - 1).half()
+    rin[torch.rand(n, 32, generator=g) < 0.05] = 0  # exact zeros
+    up = torch.randn(n, 3, generator=g) * 1e-1
+    scale = 2.0 ** 10
+    rb = grad64.rgb_backward(rin, torch.zeros(n, 32), rgb.half(), up, scale, rgb_act)
+    keep = ~rb["ambiguous"]
+    assert keep.sum() >= n - 3
+    up = up * keep[:, None]
+    rb = grad64.rgb_backward(rin, torch.zeros(n, 32), rgb.half(), up, scale, rgb_act)
+    assert (rb["fwd"]["r1"] == 0).any() and (rb["dX"] != 0).all(1).sum() > n // 2
+
+    # float64 autograd; the output derivative is taken at the rounded output o, as the kernel takes it
+    W = rgb.double().clone().requires_grad_(True)
+    X = rin.double().requires_grad_(True)
+    W1, W2, W3 = W[:2048].view(64, 32), W[2048:6144].view(64, 64), W[6144:].view(16, 64)[:3]
+    r1 = _ste16(torch.relu(X @ W1.t()))
+    r2 = _ste16(torch.relu(r1 @ W2.t()))
+    yo = r2 @ W3.t()
+    if rgb_act == 1:
+        o = grad64.f16(torch.sigmoid(yo.detach()))
+        s = o * (1 - o)
+    else:
+        s = torch.ones_like(yo)
+    (yo * s * up.double()).sum().backward()
+    got = grad64.split_dW(torch.zeros(3072, dtype=torch.float64), W.grad)
+    for k, (v, A, err) in rb["dW"].items():
+        assert (got[k] - v).abs().le(err + 1e-12 * A).all(), k
+        assert v.abs().max() > 0
+    assert (X.grad - rb["dX"]).abs().le(rb["dX_err"]).all()
+    assert (got["W3r"][3:] == 0).all() and (rb["dW"]["W3r"][0][3:] == 0).all()
+
+    # fp32 restatement at the kernel's rounding points: fp32 accumulation, fp16 activations and out-gradients
+    def r16(v): return v.half().float()
+    w = rgb.float()
+    w1, w2, w3 = w[:2048].view(64, 32), w[2048:6144].view(64, 64), w[6144:].view(16, 64)
+    x = rin.float()
+    q1 = r16(torch.relu(x @ w1.t()))
+    q2 = r16(torch.relu(q1 @ w2.t()))
+    zo = q2 @ w3[:3].t()
+    if rgb_act == 1:
+        oo = r16(torch.sigmoid(zo))
+        so = oo * (1 - oo)
+    else:
+        so = torch.ones_like(zo)
+    dout = torch.zeros(n, 16)
+    dout[:, :3] = r16(up * so * scale)
+    dr2 = r16((dout @ w3) * (q2 > 0))
+    dr1 = r16((dr2 @ w2) * (q1 > 0))
+    dX = (dr1 @ w1) * (1 / scale)
+    assert (dX.double() - rb["dX"]).abs()[keep].le(rb["dX_err"][keep]).all()
+    # the fp32 weight-gradient sums over n rows: at most n roundings of 2^-24 of the running sum
+    allow = n * 2.0 ** -24
+    fw = {"W3r": dout.t() @ q2, "W2r": dr2.t() @ q1, "W1r": dr1.t() @ x}
+    for k, (v, A, err) in rb["dW"].items():
+        assert (fw[k].double() / scale - v).abs().le(err + allow * A).all(), k
+
+
+def test_density_backward_vs_float64_autograd_and_fp32():
+    """density_backward (k_enc_bwd's chain from a scaled fp16 dL/dh) against float64 autograd of the density MLP at the
+    kernel's rounding points, and its bounds around an fp32 restatement of the kernel"""
+    enc, _ = _params(0, 51)
+    g = torch.Generator().manual_seed(52)
+    n = 300
+    feat = (torch.rand(n, 32, generator=g) * 2 - 1).half()
+    feat[:, 22:] = 0  # 11 levels: the zero-padded feature columns
+    # upstream dL/dh spread over five decades, some exact zeros, scaled as _pow2_scale does
+    dL_dh = torch.randn(n, 16, generator=g) * 10 ** (torch.rand(n, 16, generator=g) * 5 - 7)
+    dL_dh[torch.rand(n, 16, generator=g) < 0.05] = 0
+    scale = 2.0 ** math.floor(math.log2(256 / dL_dh.abs().max().item()))
+    dh, dh_err, dh_abs = grad64.scaled_dh(dL_dh, scale)
+    assert (dh.abs().max() > 128) and (dh.abs().max() <= 256)
+    db = grad64.density_backward(feat, enc[:3072].half(), dh, dh_err, dh_abs, scale)
+    keep = ~db["ambiguous"]
+    assert keep.sum() >= n - 3
+    dh, dh_err, dh_abs = dh * keep[:, None], dh_err * keep[:, None], dh_abs * keep[:, None]
+    db = grad64.density_backward(feat, enc[:3072].half(), dh, dh_err, dh_abs, scale)
+
+    W = enc[:3072].double().clone().requires_grad_(True)
+    F = feat.double().requires_grad_(True)
+    W1, W2 = W[:2048].view(64, 32), W[2048:].view(16, 64)
+    hid = _ste16(torch.relu(F @ W1.t()))
+    (hid @ W2.t() * dh / scale).sum().backward()
+    got = grad64.split_dW(W.grad, torch.zeros(7168, dtype=torch.float64))
+    for k, (v, A, err) in db["dW"].items():
+        assert (got[k] - v).abs().le(err + 1e-12 * A).all(), k
+        assert v.abs().max() > 0
+    assert (F.grad * scale - db["dfeat"]).abs().le(db["dfeat_err"]).all()
+    assert (got["W1d"][:, 22:] == 0).all() and (db["dW"]["W1d"][0][:, 22:] == 0).all()
+
+    def r16(v): return v.half().float()
+    w = enc[:3072].float()
+    w1, w2 = w[:2048].view(64, 32), w[2048:].view(16, 64)
+    x = feat.float()
+    hq = r16(torch.relu(x @ w1.t()))
+    d16 = r16(dL_dh * scale) * keep[:, None]
+    dhid = r16((d16 @ w2) * (hq > 0))
+    dfeat = r16(dhid @ w1)
+    assert (dfeat.double() - db["dfeat"]).abs()[keep].le(db["dfeat_err"][keep]).all()
+    allow = n * 2.0 ** -24
+    fw = {"W2d": d16.t() @ hq, "W1d": dhid.t() @ x}
+    for k, (v, A, err) in db["dW"].items():
+        assert (fw[k].double() / scale - v).abs().le(err + allow * A).all(), k
