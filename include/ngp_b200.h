@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 12
+#define NGP_ABI_VERSION 13
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -868,6 +868,75 @@ int ngp_points_outliers(const float* points, const uint8_t* colors, const float*
                         void* stream);
 int ngp_points_normals(const float* points, const float* views, int64_t n, int k, const int32_t* idx, float* normals,
                        void* stream);
+
+/* ----------------------------------------------------------------------------------------------
+ * Connected components (numpy + scipy restatement: oracle/components_ref.py), to remove floaters from the occupancy
+ * grid and small pieces from extracted meshes. One union-find core: parent is int32, one entry per node, the edges are
+ * generated by kernels and never stored; a link always hooks the larger root under the smaller, so a node's label is
+ * the smallest node index of its component, whatever the schedule. Sizes are exact integer counts. No float atomics:
+ * two calls are bitwise equal.
+ *
+ * Occupancy graph (ngp_grid_components): cell i = c G^3 + morton(x, y, z) of density_bitfield; cascade c has half
+ * extent mb_c = fminf(2^(c-1), scale) (fp32, the marcher's) and cell x of it spans [X_c(x), X_c(x + 1)] on an axis,
+ * X_c(x) = mb_c (2x / G - 1) in double -- exact, so every comparison below is exact.
+ *   - Shell and inner cells: a cell of cascade c >= 1 is *inner* when its closed box lies in cascade c - 1's closed box
+ *     (X_c(x) >= -mb_{c-1} and X_c(x + 1) <= mb_{c-1} on every axis); every other cell, and every cell of cascade 0, is
+ *     a *shell* cell.
+ *   - Nodes: the occupied shell cells. Edges: 26-adjacency between nodes of one cascade; and a node (x, y, z) of cascade
+ *     c >= 1 with a node (u, v, w) of cascade c - 1 when their closed boxes meet, i.e. per axis
+ *     X_{c-1}(u) <= X_c(x + 1) and X_{c-1}(u + 1) >= X_c(x). No edges between cascades further apart.
+ *   - labels (C G^3 int32): the component label of a node, -1 for every other cell (it also serves as the parent
+ *     array); sizes (C G^3 int32): at a label, the number of nodes of that component, 0 elsewhere.
+ * ngp_grid_components_clean, after ngp_components_select on those labels and sizes (n = C G^3), cascade by cascade
+ * from c = 0: an occupied shell cell is cleared iff keep[label] is 0; an occupied inner cell of cascade c is cleared
+ * iff the occupied cells of cascade c - 1 its closed box meets (by the rule of the edges) include a cleared cell and
+ * no cell left occupied. A cleared cell's bit is cleared in density_bitfield (in place) and, when density_grid (C G^3
+ * fp32) is not NULL, its value set to -1, the marker update_density_grid never revives. removed: C G^3 / 8 bytes of
+ * scratch (no initialisation). cleared (device int64[2], may be NULL): {shell cells cleared, inner cells cleared}.
+ * Both return NGP_EINVAL for a NULL pointer that is needed, G not a power of two in [2, 1024], cascades outside
+ * [1, 62], cascades G^3 >= 2^31 or scale not positive and finite. Three kernels, and one per cascade; no read-back.
+ *
+ * Selection (ngp_components_select, any graph): a component is kept iff it is among the keep_largest largest -- ranked
+ * by size descending, ties to the smaller label -- and has at least min_size nodes (keep_largest = INT64_MAX and
+ * min_size = 0 leave a criterion out). keep (n bytes): 1 at a kept label, 0 everywhere else. counts (host int64[2]):
+ * {components, kept components}. Roots compacted with a scan, sizes radix-sorted descending with the labels as values;
+ * two read-backs, so the call synchronises the stream. NGP_EINVAL for n outside [0, 2^31), a negative criterion, a
+ * NULL pointer that is needed or a short workspace; ngp_components_select_workspace(n) is about 20 n bytes plus cub's
+ * temporary storage (0 for n outside the range).
+ *
+ * Mesh graph (ngp_mesh_components): F triangles (F, 3) int64 over V vertices are connected when they share a vertex
+ * index (the marching cubes, sparse and simplified meshes share their vertices, so this is their connectivity). The
+ * nodes of the union-find are the vertices, each triangle hooking its corners; labels (F int32) = the smallest triangle
+ * index of the triangle's component and sizes (F int32) = at a label, the component's number of triangles, 0 elsewhere.
+ * Triangle indices are checked on the device (one read-back: the call synchronises the stream); an index outside
+ * [0, V) returns NGP_EINVAL. ngp_mesh_components_workspace(V, F) is about 8 V bytes.
+ * Filtering, with keep from ngp_components_select on those labels and sizes (n = F): the triangles whose label is
+ * kept, in input order, and the vertices they use, in input order, the indices renumbered. ngp_mesh_filter_count
+ * writes {V', F'} to the host int64[2] counts (one read-back); ngp_mesh_filter_emit, with the same triangles, V, F and
+ * workspace and nothing else touching the workspace in between, checks max_vertices / max_triangles against them (a
+ * read-back; NGP_EINVAL with nothing written when short) and writes out_vertices (V', 3) fp32, out_triangles (F', 3)
+ * int64, and out_normals (V', 3) fp32 / out_colors (V', 3) uint8 where both that input and that output are not NULL.
+ * ngp_mesh_filter_workspace(V, F) is about 4 (V + F) bytes plus cub's temporary storage. All mesh calls return
+ * NGP_EINVAL for V or F outside [0, 2^31), a NULL pointer that is needed or a short workspace; the workspace queries
+ * return 0 there. */
+int ngp_grid_components(const uint8_t* density_bitfield, int cascades, int grid_size, float scale, int32_t* labels,
+                        int32_t* sizes, void* stream);
+int ngp_grid_components_clean(uint8_t* density_bitfield, float* density_grid, int cascades, int grid_size, float scale,
+                              const int32_t* labels, const uint8_t* keep, uint8_t* removed, int64_t* cleared,
+                              void* stream);
+size_t ngp_components_select_workspace(int64_t n);
+int ngp_components_select(const int32_t* labels, const int32_t* sizes, int64_t n, int64_t keep_largest, int64_t min_size,
+                          uint8_t* keep, int64_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+size_t ngp_mesh_components_workspace(int64_t n_vertices, int64_t n_triangles);
+int ngp_mesh_components(const int64_t* triangles, int64_t n_vertices, int64_t n_triangles, int32_t* labels,
+                        int32_t* sizes, void* workspace, size_t workspace_bytes, void* stream);
+size_t ngp_mesh_filter_workspace(int64_t n_vertices, int64_t n_triangles);
+int ngp_mesh_filter_count(const int64_t* triangles, int64_t n_vertices, int64_t n_triangles, const int32_t* labels,
+                          const uint8_t* keep, int64_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+int ngp_mesh_filter_emit(const float* vertices, const float* normals, const uint8_t* colors, const int64_t* triangles,
+                         int64_t n_vertices, int64_t n_triangles, float* out_vertices, float* out_normals,
+                         uint8_t* out_colors, int64_t* out_triangles, int64_t max_vertices, int64_t max_triangles,
+                         void* workspace, size_t workspace_bytes, void* stream);
 
 /* ----------------------------------------------------------------------------------------------
  * Test-view images of the validation pass (reference train.py:215-221): `{idx:03d}.png` holds (rgb_pred*255).astype(np.uint8)

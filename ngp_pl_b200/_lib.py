@@ -9,7 +9,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 12  #NGP_ABI_VERSION in include/ngp_b200.h
+ABI_VERSION = 13  #NGP_ABI_VERSION in include/ngp_b200.h
 
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
@@ -247,6 +247,15 @@ SIGNATURES = {
     "ngp_points_knn": (_i, [_P, _i64, _i, _P, _P, _P, _sz, _P]),
     "ngp_points_outliers": (_i, [_P, _P, _P, _i64, _i, _P, C.c_double, _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
     "ngp_points_normals": (_i, [_P, _P, _i64, _i, _P, _P, _P]),
+    "ngp_grid_components": (_i, [_P, _i, _i, _f, _P, _P, _P]),
+    "ngp_grid_components_clean": (_i, [_P, _P, _i, _i, _f, _P, _P, _P, _P, _P]),
+    "ngp_components_select_workspace": (_sz, [_i64]),
+    "ngp_components_select": (_i, [_P, _P, _i64, _i64, _i64, _P, _P, _P, _sz, _P]),
+    "ngp_mesh_components_workspace": (_sz, [_i64, _i64]),
+    "ngp_mesh_components": (_i, [_P, _i64, _i64, _P, _P, _P, _sz, _P]),
+    "ngp_mesh_filter_workspace": (_sz, [_i64, _i64]),
+    "ngp_mesh_filter_count": (_i, [_P, _i64, _i64, _P, _P, _P, _P, _sz, _P]),
+    "ngp_mesh_filter_emit": (_i, [_P, _P, _P, _P, _i64, _i64, _P, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
     "ngp_view_images": (_i, [_P, _P, _i, _i, _P, _P, _P, _sz, _P]),
     "ngp_png_workspace": (_sz, [_i, _i]),
     "ngp_png_capacity": (_sz, [_i, _i]),

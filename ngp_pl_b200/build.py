@@ -16,7 +16,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libngp_b200.so")
 
 SOURCES = ["vren_ops.cu", "network.cu", "train.cu", "infer.cu", "modules.cu", "metrics.cu", "mesh.cu", "lpips.cu", "stage.cu", "images.cu", "jpeg.cu",
-           "texture.cu", "points.cu"]
+           "texture.cu", "points.cu", "components.cu"]
 # texture.cu's and points.cu's double arithmetic must round operation by operation as their numpy restatements
 # (oracle/mesh_texture.py, oracle/points_ref.py) do
 SOURCE_FLAGS = {"texture.cu": ["-fmad=false"], "points.cu": ["-fmad=false"]}

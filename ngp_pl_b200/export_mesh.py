@@ -1,13 +1,16 @@
 """Export the mesh of a trained checkpoint as a binary PLY, or as a textured OBJ.
 
     python -m ngp_pl_b200.export_mesh --ckpt_path ckpts/nsvf/Lego/epoch=29.ckpt [--scale 0.5] [--resolution 1024]
-        [--threshold 20] [--bounds x0 y0 z0 x1 y1 z1] [--colors] [--no_normals] [--dense] [--simplify G]
+        [--threshold 20] [--bounds x0 y0 z0 x1 y1 z1] [--colors] [--no_normals] [--dense]
+        [--keep_largest K] [--min_triangles N] [--simplify G]
         [--texture W [--texture_offset R] [--texture_samples K]] [--out mesh.ply]
 
 The checkpoint is the full or the slim one train.py writes; it is loaded into NGP(scale) with train.load_weights. By
 default the mesh is mesh.extract_mesh_sparse's: σ evaluated and marching cubes run only near the cells the model's
 occupancy grid marks, so 2048^3 and 4096^3 lattices fit in memory. --dense gives mesh.extract_mesh's mesh of the whole
 lattice (the notebook's mesh cell): a different mesh, which also has the surfaces the occupancy grid has culled.
+--keep_largest K / --min_triangles N drop the pieces of the mesh (triangles sharing vertices) that are not among the K
+largest or have fewer than N triangles, with mesh.remove_small_components: floaters and the shells of closed cavities.
 --simplify G then reduces the mesh with mesh.simplify_mesh on a G^3 cluster grid over the lattice box (vertex
 clustering with quadric-error placement; colours become the means of each cluster's colours).
 --texture W bakes the model's colours into a W x W atlas with mesh.bake_texture and writes --out (which must end in
@@ -34,6 +37,10 @@ def get_parser():
     p.add_argument("--colors", action="store_true", help="vertex colours from the model, seen head-on")
     p.add_argument("--no_normals", action="store_true", help="leave the normals out of the PLY")
     p.add_argument("--dense", action="store_true", help="the unculled mesh of the whole lattice (mesh.extract_mesh)")
+    p.add_argument("--keep_largest", type=int, default=None, metavar="K",
+                   help="keep only the K largest connected pieces of the mesh (by triangle count), >= 1")
+    p.add_argument("--min_triangles", type=int, default=None, metavar="N",
+                   help="drop the connected pieces of the mesh with fewer than N triangles, >= 1")
     p.add_argument("--simplify", type=int, default=None, metavar="G",
                    help="simplify on a G^3 cluster grid over the lattice box before writing, 1..65536")
     p.add_argument("--texture", type=int, default=None, metavar="W",
@@ -63,6 +70,10 @@ def check_args(args, parser):
         lo, hi = args.bounds[:3], args.bounds[3:]
         if not all(math.isfinite(v) for v in args.bounds) or any(a >= b for a, b in zip(lo, hi)):
             parser.error("--bounds: every lower corner coordinate must be below the upper one")
+    if args.keep_largest is not None and args.keep_largest < 1:
+        parser.error("--keep_largest must be >= 1")
+    if args.min_triangles is not None and args.min_triangles < 1:
+        parser.error("--min_triangles must be >= 1")
     if args.simplify is not None and not 1 <= args.simplify <= 65536:
         parser.error("--simplify must be in 1..65536")
     if args.texture is not None:
@@ -137,6 +148,12 @@ def main(argv=None):
     if stats is not None:
         line += " (bricks: %d active, %d visited, %d surface)" % (stats["active"], stats["visited"], stats["surface"])
     box = bounds if bounds is not None else (model._xyz_min_host, model._xyz_max_host)
+    if args.keep_largest is not None or args.min_triangles is not None:
+        t0 = time.perf_counter()
+        m, cs = mesh.remove_small_components(m, args.keep_largest, args.min_triangles, return_stats=True)
+        torch.cuda.synchronize()
+        line += "; kept %d of %d pieces, %d vertices, %d triangles in %.3f s" % (
+            cs["kept"], cs["components"], m["vertices"].shape[0], m["triangles"].shape[0], time.perf_counter() - t0)
     if args.simplify is not None:
         t0 = time.perf_counter()
         m = mesh.simplify_mesh(m, args.simplify, box)

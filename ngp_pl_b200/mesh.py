@@ -8,6 +8,9 @@ PyMCubes, trimesh or scikit-image.
     extract_mesh_sparse(model, resolution=1024, bounds=None, threshold=20.0, normals=True, colors=False,
                         return_stats=False)                       the mesh of σ where the occupancy grid allows a surface
     simplify_mesh(mesh, grid, bounds=None)                        vertex clustering with quadric-error placement
+    mesh_components(mesh)                                         component label and size per triangle
+    remove_small_components(mesh, keep_largest=None, min_triangles=None, return_stats=False)
+                                                                  the mesh without its small pieces
     bake_texture(model, mesh, size=4096, offset=0.0, samples=16, return_texels=False)
                                                                   a per-triangle texture atlas and its colours
     write_ply(path, vertices, triangles, normals=None, colors=None) binary little-endian PLY, numpy only
@@ -27,6 +30,10 @@ the bricks a surface passes through; its cost and memory follow the occupied vol
 simplify_mesh (`ngp_mesh_simplify_count` / `_emit`) reduces a mesh to at most one vertex per cell of a grid^3 cluster
 grid, placed where the cell's triangle planes meet (quadric error), so thin parts and sharp edges a coarser lattice
 would lose keep their place at a fraction of the triangle count.
+
+mesh_components / remove_small_components (`ngp_mesh_components`, `ngp_components_select`, `ngp_mesh_filter_count` /
+`_emit` in csrc/components.cu) split a mesh into the pieces that share vertices, on the device, and keep the large ones:
+floaters and the closed shells of cavities no ray reaches go, whichever extraction made the mesh.
 
 bake_texture (`ngp_mesh_texture_atlas` / `_texels` / `_bake` in csrc/texture.cu) gives every triangle its own square
 of a texture atlas and bakes the model's colours into it through the fused forward, so a simplified mesh keeps the
@@ -370,6 +377,101 @@ def simplify_mesh(mesh, grid, bounds=None):
                        "ngp_mesh_simplify_emit")
         del ws
     return {"vertices": out_v, "triangles": out_t, "normals": out_n, "colors": out_c}
+
+
+def _mesh_in(mesh, fn):
+    verts, tris = mesh["vertices"], mesh["triangles"]
+    nrm, col = mesh.get("normals"), mesh.get("colors")
+    for t in (verts, tris, nrm, col):
+        if t is not None:
+            _chk(t, fn)
+    verts = verts.detach().to(torch.float32).reshape(-1, 3).contiguous()
+    tris = tris.detach().to(torch.int64).reshape(-1, 3).contiguous()
+    V = verts.shape[0]
+    if nrm is not None:
+        nrm = nrm.detach().to(torch.float32).reshape(-1, 3).contiguous()
+    if col is not None:
+        col = col.detach().to(torch.uint8).reshape(-1, 3).contiguous()
+    for t, what in ((nrm, "normals"), (col, "colors")):
+        if t is not None and t.shape[0] != V:
+            raise RuntimeError("ngp_pl_b200.mesh.%s: %d %s for %d vertices" % (fn, t.shape[0], what, V))
+    return verts, tris, nrm, col
+
+
+def _components(tris, V, fn):
+    F = tris.shape[0]
+    dev = tris.device
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        ws_bytes = L.ngp_mesh_components_workspace(V, F)
+        if ws_bytes == 0:
+            raise RuntimeError("ngp_pl_b200.mesh.%s: %d vertices and %d triangles: both must be below 2^31" % (fn, V, F))
+        _need(dev, ws_bytes + F * 8, "the components of %d vertices and %d triangles" % (V, F), fn)
+        ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+        labels = torch.empty(F, device=dev, dtype=torch.int32)
+        sizes = torch.empty(F, device=dev, dtype=torch.int32)
+        rc = L.ngp_mesh_components(tris.data_ptr(), V, F, labels.data_ptr(), sizes.data_ptr(), ws.data_ptr(), ws_bytes,
+                                   _st(dev))
+        if rc == -22 and F > 0:
+            raise RuntimeError("ngp_pl_b200.mesh.%s: a triangle index lies outside [0, %d)" % (fn, V))
+        _lib.check(rc, "ngp_mesh_components")
+    return labels, sizes
+
+
+@torch.no_grad()
+def mesh_components(mesh):
+    """Connected components of a mesh dict as extract_mesh / extract_mesh_sparse / simplify_mesh return it: triangles
+    that share a vertex index are connected. Returns (labels, sizes), (F,) int32 each on the mesh's device: labels[t] =
+    the smallest triangle index of t's component, sizes[l] = the number of triangles of the component labelled l (0 at
+    every index that is not a label). RuntimeError for CPU tensors, V or F >= 2^31 or a triangle index outside [0, V).
+    Deterministic: two calls are bitwise equal."""
+    verts, tris, _, _ = _mesh_in(mesh, "mesh_components")
+    return _components(tris, verts.shape[0], "mesh_components")
+
+
+@torch.no_grad()
+def remove_small_components(mesh, keep_largest=None, min_triangles=None, return_stats=False):
+    """The mesh without the components that are not among the keep_largest largest (by triangle count, ties to the
+    smaller label) or have fewer than min_triangles triangles; at least one criterion is required, and with both a
+    component must pass both. Kept triangles stay in input order with their corner order, the vertices they use stay in
+    input order and are renumbered; normals and colours go with their vertices. Returns a dict with the same keys as
+    the input (a mesh nothing is removed from comes back bitwise); return_stats=True also returns {'components', 'kept'}.
+    RuntimeError as mesh_components, and before allocating when the output does not fit in free device memory."""
+    from .components import criterion, select_components
+    fn = "mesh.remove_small_components"
+    keep_largest = criterion(keep_largest, "keep_largest", fn)
+    min_triangles = criterion(min_triangles, "min_triangles", fn)
+    if keep_largest is None and min_triangles is None:
+        raise RuntimeError("ngp_pl_b200.%s: give keep_largest, min_triangles, or both" % fn)
+    verts, tris, nrm, col = _mesh_in(mesh, "remove_small_components")
+    V, F = verts.shape[0], tris.shape[0]
+    dev = verts.device
+    labels, sizes = _components(tris, V, "remove_small_components")
+    keep, stats = select_components(labels, sizes, keep_largest, min_triangles, fn)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        ws_bytes = L.ngp_mesh_filter_workspace(V, F)
+        _need(dev, ws_bytes, "the filter workspace of %d vertices and %d triangles" % (V, F), "remove_small_components")
+        ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
+        st = _st(dev)
+        tot = (C.c_int64 * 2)()
+        _lib.check(L.ngp_mesh_filter_count(tris.data_ptr(), V, F, labels.data_ptr(), keep.data_ptr(), tot, ws.data_ptr(),
+                                           ws_bytes, st), "ngp_mesh_filter_count")
+        del labels, sizes, keep
+        nv, nt = int(tot[0]), int(tot[1])
+        _need(dev, nv * (12 + (12 if nrm is not None else 0) + (3 if col is not None else 0)) + nt * 24,
+              "%d vertices and %d triangles" % (nv, nt), "remove_small_components")
+        out_v = torch.empty(nv, 3, device=dev, dtype=torch.float32)
+        out_t = torch.empty(nt, 3, device=dev, dtype=torch.int64)
+        out_n = torch.empty(nv, 3, device=dev, dtype=torch.float32) if nrm is not None else None
+        out_c = torch.empty(nv, 3, device=dev, dtype=torch.uint8) if col is not None else None
+        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        _lib.check(L.ngp_mesh_filter_emit(verts.data_ptr(), ptr(nrm), ptr(col), tris.data_ptr(), V, F, out_v.data_ptr(),
+                                          ptr(out_n), ptr(out_c), out_t.data_ptr(), nv, nt, ws.data_ptr(), ws_bytes, st),
+                   "ngp_mesh_filter_emit")
+        del ws
+    m = {"vertices": out_v, "triangles": out_t, "normals": out_n, "colors": out_c}
+    return (m, stats) if return_stats else m
 
 
 def texture_size_for(n_triangles):
