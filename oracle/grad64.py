@@ -18,7 +18,7 @@ Every value comes with a rigorous bound of how far the kernel's may lie from it 
   * the forward values the kernel may round the other way: where an activation's fp32 accumulation error straddles an
     fp16 rounding boundary, the kernel's value may be one ulp off; that difference is carried one layer on, into the next
     layer's ReLU masks, the sigmoid derivative, exp(h0) and the weight gradients' inputs. (A flip caused by another
-    flip -- two rare events in one row -- is not modelled.)
+    flip is modelled only with carry=True, which follows every flip to the forward's outputs.)
 A row whose ReLU masks are not determined by those intervals is flagged in `ambiguous`: there the kernel and the
 reference may take different branches and no rounding bound applies. `ambiguous_own` flags the subset where the
 pre-activation's own accumulation error alone (|z| <= 2^-20 sum|terms|) leaves the mask open.
@@ -187,19 +187,21 @@ def mlp_forward(feat, sh, enc_mlp, rgb_params, rgb_act=1, carry=False, d_feat=No
     return f
 
 
-def rgb_backward(rin, d_rin, rgb_params, up_rgb, scale, rgb_act=1):
+def rgb_backward(rin, d_rin, rgb_params, up_rgb, scale, rgb_act=1, carry=False):
     """k_mlp_rgb_bwd's chain from fp16 inputs rin (n, 32) the kernel may hold differently by up to d_rin (0 when they are
     the kernel's own input), fp32 upstream gradients up_rgb (n, 3) and the power-of-two loss scale:
       dout = fp16(up o (1 - o) scale),  dr2 = fp16([r2 > 0] dout W3r),  dr1 = fp16([r1 > 0] dr2 W2r)
       dX   = (dr1 W1r) / scale in fp32: all 32 columns, no fp16 rounding
     Returns a dict: dX (n, 32, unscaled), dX_err (its bound: the operand errors and the fp32 accumulation of dr1 W1r,
     plus one fp32 rounding), dX_abs; dout / dr2 / dr1 with _err / _abs (scaled); dW {W3r, W2r, W1r: (value, A, err)}
-    (unscaled); ambiguous / ambiguous_own (n) bool; the forward dict `fwd` (rgb_forward's)."""
+    (unscaled); ambiguous / ambiguous_own (n) bool; the forward dict `fwd` (rgb_forward's). carry: the forward's bounds
+    carry what d_rin and every earlier flip move each layer by (rgb_forward(carry=True)), and so do the masks, the sigmoid
+    derivative and the weight gradients' inputs that depend on them."""
     dt = torch.float64
     Wr = rgb_params.to(dt)
     W1r, W2r, W3r = Wr[:2048].view(64, 32), Wr[2048:6144].view(64, 64), Wr[6144:7168].view(16, 64)
     up_rgb = up_rgb.to(dt)
-    f = rgb_forward(rin, d_rin, rgb_params, rgb_act)
+    f = rgb_forward(rin, d_rin, rgb_params, rgb_act, carry)
     rin, d_rin, r1, d_r1, r2, d_r2, yo = f["rin"], f["d_rin"], f["r1"], f["d_r1"], f["r2"], f["d_r2"], f["yo"]
     n = rin.shape[0]
     if rgb_act == 1:
@@ -259,13 +261,18 @@ def density_backward(feat, enc_mlp, dh, dh_err, dh_abs, scale):
                 dW=dW, hid=hid, d_hid=d_hid, ambiguous=amb[0], ambiguous_own=amb[1])
 
 
-def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1):
+def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1, carry=False):
     """feat (n, 32) fp16 features, sh (n, 16) float64 SH-4 (unrounded), enc_mlp (>= 3072) / rgb_params (7168) fp16 weights,
     up_sig (n), up_rgb (n, 3) fp32 upstream gradients, scale the power-of-two loss scale (a number).
     Returns a dict: dfeat (n, 32, scaled by `scale`, like the kernel's workspace), dfeat_err, dfeat_abs, ambiguous (n) bool,
     dW {name: (value, A, err)} for W3r, W2r, W1r, W2d, W1d (unscaled), and the forward activations.
     It is rgb_backward, then the sum k_ngp_bwd3 rounds once: dh = fp16(dr1 W1r[:, 16:] + up_sig exp(h0) scale in
-    column 0), then density_backward."""
+    column 0), then density_backward.
+    carry=False models one flip per row: an activation may round the other way where its own accumulation error
+    straddles a boundary, and that flip reaches the next layer only. carry=True follows every flip to the end of the
+    forward (mlp_forward(carry=True)): a flip of hid moves h, which may move h0 by an ulp (and exp(h0) with it) or flip a
+    ReLU mask of the colour net. The values are the same; the bounds and the undecided rows can only grow. Trained
+    weights, whose out-gradients cancel heavily, need it."""
     dt = torch.float64
     feat = feat.to(dt)
     Wr = rgb_params.to(dt)
@@ -273,13 +280,13 @@ def mlp_backward(feat, sh, enc_mlp, rgb_params, up_sig, up_rgb, scale, rgb_act=1
     up_sig = up_sig.to(dt)
 
     # ---- forward recompute with the kernel's rounding points, as intervals ----
-    f = mlp_forward(feat, sh, enc_mlp, rgb_params, rgb_act)
+    f = mlp_forward(feat, sh, enc_mlp, rgb_params, rgb_act, carry)
     hid, h, d_h, rin, r1, r2, yo = f["hid"], f["h"], f["d_h"], f["rin"], f["r1"], f["r2"], f["yo"]
     if rgb_act == 1:
         o = f["out"]
 
     # ---- out-gradient chain ----
-    rb = rgb_backward(rin, f["d_rin"], rgb_params, up_rgb, scale, rgb_act)
+    rb = rgb_backward(rin, f["d_rin"], rgb_params, up_rgb, scale, rgb_act, carry)
     dout, dr2, dr1, dr1_err, dr1_abs = rb["dout"], rb["dr2"], rb["dr1"], rb["dr1_err"], rb["dr1_abs"]
     Wh = W1r[:, 16:]
     y, a, e = dr1 @ Wh, dr1_abs @ Wh.abs(), dr1_err @ Wh.abs()

@@ -5,6 +5,8 @@ silently agree with a wrong kernel (tests/test_backward_fp64_gpu.py compares the
   * its feat_save decoder against a plain encoder of the documented fragment layout;
   * its two halves, rgb_backward and density_backward (the stand-alone module kernels' chains), against float64 autograd
     at the kernels' rounding points, and their bounds around an fp32 restatement of the kernels;
+  * mlp_backward(carry=True), whose bounds follow every forward flip to the end: the same values as the one-flip model,
+    bounds and undecided rows that contain it, and a fp32 restatement of k_ngp_bwd3 inside its bounds;
   * mlp_backward against its own stored outputs (tests/golden/grad64_mlp_backward.npz), so that a change to the forward
     it shares with mlp_forward shows.
 """
@@ -383,3 +385,81 @@ def test_density_backward_vs_float64_autograd_and_fp32():
     fw = {"W2d": d16.t() @ hq, "W1d": dhid.t() @ x}
     for k, (v, A, err) in db["dW"].items():
         assert (fw[k].double() / scale - v).abs().le(err + allow * A).all(), k
+
+
+@pytest.mark.parametrize("rgb_act", [1, 0])
+def test_mlp_backward_carry_contains_one_flip_model_and_fp32(oracle, rgb_act):
+    """mlp_backward(carry=True) has mlp_backward's values; its bounds and undecided rows contain the one-flip model's;
+    and an fp32 restatement of k_ngp_bwd3's chain (fp32 accumulation, fp16 activations and out-gradients, fp32 SH of the
+    normalised direction) lies inside its bounds on every decided row, its weight gradients inside the carried
+    weight-gradient bounds; and carry does widen the bounds"""
+    from oracle.oracle import torch_sh4
+    meta, total = oracle.grid_meta(16, 19, 16, float(np.float32(np.exp(np.log(2048 * 0.5 / 16) / 15))))
+    enc, rgb = _params(total, 51)
+    n = 3000
+    x, d = _points(n, 52)
+    x01 = x + 0.5
+    with torch.no_grad():
+        feat = oracle.torch_grid_encode(meta, enc[3072:].view(-1, 2), x01).half()
+    g = torch.Generator().manual_seed(53)
+    up_sig = torch.randn(n, generator=g) * 1e-2
+    up_rgb = torch.randn(n, 3, generator=g) * 1e-1
+    scale = 2.0 ** 8
+    args = (feat, grad64.sh4_64(d), enc[:3072].half(), rgb.half(), up_sig, up_rgb, scale, rgb_act)
+    one, car = grad64.mlp_backward(*args), grad64.mlp_backward(*args, carry=True)
+    for k in ("dfeat", "hid", "h", "rin", "r1", "r2", "o"):
+        assert torch.equal(one[k], car[k]), k
+    assert (car["dfeat_err"] >= one["dfeat_err"]).all()
+    assert (car["ambiguous"] | ~one["ambiguous"]).all() and car["ambiguous"].double().mean() < 0.1
+    for k, (v, A, err) in car["dW"].items():
+        v1, A1, err1 = one["dW"][k]
+        assert torch.equal(v, v1) and torch.equal(A, A1) and (err >= err1).all(), k
+
+    def r16(v): return v.half().float()
+    w, wr = enc[:3072].float(), rgb.float()
+    w1d, w2d = w[:2048].view(64, 32), w[2048:3072].view(16, 64)
+    w1r, w2r, w3r = wr[:2048].view(64, 32), wr[2048:6144].view(64, 64), wr[6144:].view(16, 64)
+    hid = r16(torch.relu(feat.float() @ w1d.t()))
+    h = r16(hid @ w2d.t())
+    dn = d / torch.sqrt((d * d).sum(1, keepdim=True))
+    rin = torch.cat([r16(torch_sh4(dn)), h], 1)
+    q1 = r16(torch.relu(rin @ w1r.t()))
+    q2 = r16(torch.relu(q1 @ w2r.t()))
+    zo = q2 @ w3r[:3].t()
+    oo = r16(torch.sigmoid(zo)) if rgb_act == 1 else zo
+    so = oo * (1 - oo) if rgb_act == 1 else torch.ones_like(zo)
+    dout = torch.zeros(n, 16)
+    dout[:, :3] = r16(up_rgb * so * scale)
+    dr2 = r16((dout @ w3r) * (q2 > 0))
+    dr1 = r16((dr2 @ w2r) * (q1 > 0))
+    c = dr1 @ w1r[:, 16:]
+    c[:, 0] += up_sig * torch.exp(h[:, 0].clamp(-15, 15)) * scale
+    dh = r16(c)
+    dhid = r16((dh @ w2d) * (hid > 0))
+    dfeat = r16(dhid @ w1d)
+    keep = ~car["ambiguous"]
+    assert ((dfeat.double() - car["dfeat"]).abs() <= car["dfeat_err"])[keep].all()
+    # carry widens something: more undecided rows, and wider bounds of the feature and weight gradients
+    assert car["ambiguous"].sum() > one["ambiguous"].sum()
+    assert (car["dfeat_err"] > one["dfeat_err"]).any()
+    assert any((car["dW"][k][2] > one["dW"][k][2]).any() for k in car["dW"])
+
+    # the weight gradients of the fp32 restatement, over the rows the carried model decides (the others get no
+    # upstream gradient): within the carried bound plus the fp32 sums' n roundings of 2^-24 of the absolute sum
+    up_sig, up_rgb = up_sig * keep, up_rgb * keep[:, None]
+    car = grad64.mlp_backward(feat, grad64.sh4_64(d), enc[:3072].half(), rgb.half(), up_sig, up_rgb, scale, rgb_act,
+                              carry=True)
+    assert not car["ambiguous"][keep].any()
+    dout = torch.zeros(n, 16)
+    dout[:, :3] = r16(up_rgb * so * scale)
+    dr2 = r16((dout @ w3r) * (q2 > 0))
+    dr1 = r16((dr2 @ w2r) * (q1 > 0))
+    c = dr1 @ w1r[:, 16:]
+    c[:, 0] += up_sig * torch.exp(h[:, 0].clamp(-15, 15)) * scale
+    dh = r16(c)
+    dhid = r16((dh @ w2d) * (hid > 0))
+    fw = {"W3r": dout.t() @ q2, "W2r": dr2.t() @ q1, "W1r": dr1.t() @ rin, "W2d": dh.t() @ hid,
+          "W1d": dhid.t() @ feat.float()}
+    for k, (v, A, err) in car["dW"].items():
+        assert (fw[k].double() / scale - v).abs().le(err + n * 2.0 ** -24 * A).all(), k
+        assert v.abs().max() > 0, k
