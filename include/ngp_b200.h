@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 13
+#define NGP_ABI_VERSION 14
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -868,6 +868,65 @@ int ngp_points_outliers(const float* points, const uint8_t* colors, const float*
                         void* stream);
 int ngp_points_normals(const float* points, const float* views, int64_t n, int k, const int32_t* idx, float* normals,
                        void* stream);
+
+/* ----------------------------------------------------------------------------------------------
+ * Depth fusion (TSDF): depth maps rendered from the training views (or any others) fused into a truncated signed
+ * distance field on a lattice, and its mesh. A TSDF mesh holds only surfaces the cameras saw: no cavity no ray reaches,
+ * and no sigma threshold. numpy restatement: oracle/tsdf_ref.py (np.float32, bit for bit).
+ *
+ * Lattice: an NgpLattice as mesh.lattice(resolution, lo, hi) builds it (the points of ngp_density_lattice). State per
+ * point p (linear index): tsdf F (fp32), weight W (int32, the number of observations), color (3 fp32, a mean) and
+ * color_weight Wc (int32) -- 24 B. Initial state: all 0.
+ * Views: poses (n_views, 3, 4) fp32, R | o with the loaders' [right down front] axes; one pinhole K (3x3 fp32, host,
+ * row-major: fx = K[0], cx = K[2], fy = K[4], cy = K[5]) and W x H pixels; directions (H W, 3) fp32, the table
+ * datasets.ray_directions builds from that K (camera-frame z = 1); per view and pixel depth, opacity (fp32) and rgb
+ * (3 fp32) as ngp_render_infer_frame writes them. t = depth / opacity is the ray parameter along the unnormalised
+ * direction, i.e. the camera-frame z of the surface.
+ *
+ * One observation of point x (x_a = lo[a] + (float)idx_a step[a], multiply then add) by view v, views in pose order;
+ * the view is skipped as soon as a condition fails. Every fp32 operation is rounded on its own (no contraction), sums
+ * left to right:
+ *   1. d = x - o; (xc, yc, zc) = R^T d, component c = (R[0][c] d0 + R[1][c] d1) + R[2][c] d2. Require zc > 0.
+ *   2. px = (fx xc) / zc + cx, py = (fy yc) / zc + cy. Require 0 <= px < W and 0 <= py < H (NaN fails); pixel
+ *      u = floor(px), v = floor(py): the pixel whose direction passes nearest.
+ *   3. op = opacity of the pixel; require op >= min_opacity (NaN fails); t = depth / op, required finite.
+ *   4. |dir| = sqrt((dx dx + dy dy) + dz dz) of the pixel's direction; sdf = (t - zc) |dir|. Require sdf >= -trunc.
+ *   5. f = fminf(1, sdf / trunc); F <- (F (float)W + f) / (float)(W + 1); W <- W + 1.
+ *   6. Only if sdf <= trunc: per channel c = fminf(rgb / op, 1) (the colour rule of the point-cloud export);
+ *      color <- (color (float)Wc + c) / (float)(Wc + 1); Wc <- Wc + 1.
+ * There are no float atomics, and the result does not depend on how the views are split into calls: two calls are
+ * bitwise equal, and views integrated one call at a time give the result of one call with all of them.
+ *
+ * ngp_tsdf_integrate applies n_views views to the state in place, NGP_TSDF_GROUP views per launch (each launch reads
+ * and writes a point's 24 B at most once: the state traffic is at most 2 * 24 * N * ceil(n_views / NGP_TSDF_GROUP)
+ * bytes for N points). depth / opacity (n_views, H W), rgb (n_views, H W, 3). NGP_EINVAL for a NULL pointer that is
+ * needed, n[a] < 1, trunc not positive and finite, min_opacity outside (0, 1], n_views < 0, W or H < 1 or W H >= 2^31.
+ * No read-back.
+ *
+ * Masked marching cubes (the TSDF mesh): the rules of ngp_marching_cubes_* on v = -F at iso 0, except at unobserved
+ * points (W = 0):
+ *   - a point is inside iff it is observed and F < 0; an edge is crossed iff both ends are observed and exactly one
+ *     is inside;
+ *   - a cell emits triangles iff its 8 corners are observed;
+ *   - a vertex exists iff its edge is crossed and one of the cells around the edge emits (every crossed edge of a cell
+ *     is used by the case table, so no vertex is left unreferenced); vertex order is still (linear index of p, a);
+ *   - normals: the dense gradient rule, a neighbour with W = 0 treated like one past the lattice border (one-sided
+ *     difference, 0 when neither neighbour along the axis is observed);
+ *   - colours (optional, (V, 3) uint8): the colour means of the edge's ends interpolated with the vertex's t, c0 + t
+ *     (c1 - c0), when both have Wc > 0, else the inside end's mean (it has Wc >= 1); rint(255 c) clamped to 0..255.
+ * So a volume observed everywhere gives exactly ngp_marching_cubes_* of -F at iso 0. The protocol, workspace and
+ * refusals are those of ngp_marching_cubes_count / _emit (ngp_tsdf_mc_workspace is ngp_marching_cubes_workspace);
+ * emit also refuses colors without color / color_weight. */
+#define NGP_TSDF_GROUP 64
+int ngp_tsdf_integrate(const NgpLattice* lat, float trunc, int n_views, const float* poses, const float* K, int W, int H,
+                       const float* directions, const float* depth, const float* opacity, const float* rgb,
+                       float min_opacity, float* tsdf, int32_t* weight, float* color, int32_t* color_weight, void* stream);
+size_t ngp_tsdf_mc_workspace(const NgpLattice* lat);
+int ngp_tsdf_mc_count(const float* tsdf, const int32_t* weight, const NgpLattice* lat, int64_t* counts, void* workspace,
+                      size_t workspace_bytes, void* stream);
+int ngp_tsdf_mc_emit(const float* tsdf, const int32_t* weight, const float* color, const int32_t* color_weight,
+                     const NgpLattice* lat, float* vertices, float* normals, uint8_t* colors, int64_t* triangles,
+                     int64_t max_vertices, int64_t max_triangles, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ----------------------------------------------------------------------------------------------
  * Connected components (numpy + scipy restatement: oracle/components_ref.py), to remove floaters from the occupancy

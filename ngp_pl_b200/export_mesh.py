@@ -4,6 +4,7 @@
         [--threshold 20] [--bounds x0 y0 z0 x1 y1 z1] [--colors] [--no_normals] [--dense]
         [--keep_largest K] [--min_triangles N] [--simplify G]
         [--texture W [--texture_offset R] [--texture_samples K]] [--out mesh.ply]
+        [--tsdf --root_dir R [--dataset_name nerf|colmap] [--downsample 1.0] [--min_opacity 0.5] [--tsdf_trunc T]]
 
 The checkpoint is the full or the slim one train.py writes; it is loaded into NGP(scale) with train.load_weights. By
 default the mesh is mesh.extract_mesh_sparse's: σ evaluated and marching cubes run only near the cells the model's
@@ -17,6 +18,12 @@ clustering with quadric-error placement; colours become the means of each cluste
 .obj) with mesh.write_obj, next to its .mtl and .png. The bake renders --texture_samples samples along each texel's
 inward normal from --texture_offset outside the surface: by default the cluster cell with --simplify, where vertices
 sit up to sqrt(3) cells off the surface they stand for, and the largest lattice step without it.
+--tsdf gives fusion.extract_mesh_tsdf's mesh instead: every pixel of the training views of --root_dir (cameras from
+datasets.scene_meta(--dataset_name, --root_dir, 'train', --downsample), metadata only, no image decoded) rendered with a
+black background, the depth of the pixels of opacity >= --min_opacity fused into a truncated signed distance field on
+the --resolution lattice over --bounds (truncation --tsdf_trunc, default 4 lattice steps), and its masked marching
+cubes: only surfaces the cameras saw, no σ threshold. --colors then writes the fused colours. The state takes 24 B per
+lattice point, so --tsdf takes --resolution up to 1024.
 Bad arguments are refused with exit status 2 before torch is imported.
 """
 import argparse
@@ -50,6 +57,14 @@ def get_parser():
                         "with --simplify, else the largest lattice step)")
     p.add_argument("--texture_samples", type=int, default=16, metavar="K", help="samples per texel, 1..256")
     p.add_argument("--out", type=str, default="mesh.ply", help="output PLY path (.obj with --texture)")
+    p.add_argument("--tsdf", action="store_true",
+                   help="fuse the training views' rendered depth into a TSDF and mesh it (fusion.extract_mesh_tsdf)")
+    p.add_argument("--root_dir", type=str, default=None, help="with --tsdf: the scene the model was trained on (its cameras)")
+    p.add_argument("--dataset_name", type=str, default="nerf", choices=["nerf", "colmap"])
+    p.add_argument("--downsample", type=float, default=1.0, help="image downsample of the cameras, in (0, 1]")
+    p.add_argument("--min_opacity", type=float, default=0.5, help="with --tsdf: opacity a pixel needs to count, in (0, 1]")
+    p.add_argument("--tsdf_trunc", type=float, default=None, metavar="T",
+                   help="with --tsdf: truncation distance in world units, > 0 (default: 4 lattice steps)")
     return p
 
 
@@ -87,6 +102,20 @@ def check_args(args, parser):
         parser.error("--texture_offset must be >= 0 and finite")
     if not 1 <= args.texture_samples <= 256:
         parser.error("--texture_samples must be in 1..256")
+    if not (0 < args.downsample <= 1):
+        parser.error("--downsample must be in (0, 1]")
+    if not (0 < args.min_opacity <= 1):
+        parser.error("--min_opacity must be in (0, 1]")
+    if args.tsdf_trunc is not None and not (args.tsdf_trunc > 0 and math.isfinite(args.tsdf_trunc)):
+        parser.error("--tsdf_trunc must be positive and finite")
+    if args.tsdf:
+        if args.root_dir is None:
+            parser.error("--tsdf needs --root_dir: the fusion projects through the cameras' K and image size, which a "
+                         "checkpoint does not store")
+        if args.dense:
+            parser.error("--tsdf and --dense exclude each other")
+        if args.resolution > 1024:
+            parser.error("--resolution must be at most 1024 with --tsdf (24 B of state per lattice point)")
     return args
 
 
@@ -135,9 +164,16 @@ def main(argv=None):
     normals = not args.no_normals
     torch.cuda.synchronize()
     t0 = time.perf_counter()
-    if args.dense:
+    stats = None
+    if args.tsdf:
+        from . import datasets, fusion
+        meta = datasets.scene_meta(args.dataset_name, args.root_dir, "train", args.downsample)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        m = fusion.extract_mesh_tsdf(model, torch.as_tensor(meta.poses), meta.K, meta.img_wh, args.resolution, bounds,
+                                     args.tsdf_trunc, args.min_opacity, normals=normals, colors=args.colors)
+    elif args.dense:
         m = mesh.extract_mesh(model, args.resolution, bounds, args.threshold, normals=normals, colors=args.colors)
-        stats = None
     else:
         m, stats = mesh.extract_mesh_sparse(model, args.resolution, bounds, args.threshold, normals=normals,
                                             colors=args.colors, return_stats=True)
