@@ -120,21 +120,41 @@ __device__ __forceinline__ float2 grid_lookup(const uint32_t* __restrict__ table
 // pair does not straddle the wrap). The scatter uses that: one 16-byte red.global.add.v4.f32 instead of two 8-byte ones
 // (one L2 atomic transaction). The same trick in the GATHER (aligned 8-byte pair load + predicated load of the unpaired
 // corner) and a software-pipelined gather were slower than the plain eight 4-byte loads and are not kept.
-// the 8 corner contributions acc[2k], acc[2k+1] of one cell into the gradient table of a level, x-pairs merged when aligned
-__device__ __forceinline__ void grid_scatter_cell_paired(const float* lvl /* level base, float2 per entry */, const uint32_t (&idx)[8],
-                                                         const float (&acc)[16]) {
+// the corner contributions acc[2k], acc[2k+1] of one cell that the bit mask `own` selects into the gradient table of a
+// level, x-pairs merged when both are owned and aligned
+__device__ __forceinline__ void grid_scatter_cell_owned(const float* lvl /* level base, float2 per entry */, const uint32_t (&idx)[8],
+                                                        const float (&acc)[16], uint32_t own) {
 #pragma unroll
     for (int k = 0; k < 8; k += 2) {
-        if ((idx[k] ^ idx[k + 1]) == 1u) {
+        const bool o0 = (own >> k) & 1u, o1 = (own >> (k + 1)) & 1u;
+        if (o0 && o1 && (idx[k] ^ idx[k + 1]) == 1u) {
             float* p = const_cast<float*>(reinterpret_cast<const float*>(entry_ptr<8>(lvl, idx[k] & ~1u)));
             if (idx[k] & 1u) red_add_f32x4(p, acc[2 * k + 2], acc[2 * k + 3], acc[2 * k], acc[2 * k + 1]);
             else red_add_f32x4(p, acc[2 * k], acc[2 * k + 1], acc[2 * k + 2], acc[2 * k + 3]);
         } else {
-            red_add_f32x2(const_cast<float*>(reinterpret_cast<const float*>(entry_ptr<8>(lvl, idx[k]))), acc[2 * k], acc[2 * k + 1]);
-            red_add_f32x2(const_cast<float*>(reinterpret_cast<const float*>(entry_ptr<8>(lvl, idx[k + 1]))), acc[2 * k + 2],
-                          acc[2 * k + 3]);
+            if (o0)
+                red_add_f32x2(const_cast<float*>(reinterpret_cast<const float*>(entry_ptr<8>(lvl, idx[k]))), acc[2 * k], acc[2 * k + 1]);
+            if (o1)
+                red_add_f32x2(const_cast<float*>(reinterpret_cast<const float*>(entry_ptr<8>(lvl, idx[k + 1]))), acc[2 * k + 2],
+                              acc[2 * k + 3]);
         }
     }
+}
+
+// Corners two cells share. Corner k = dx + 2*dy + 4*dz of cell c is the grid vertex c + (dx, dy, dz); if the cell
+// c + d is adjacent (every |d_i| <= 1), that vertex is its corner k - (d.x + 2*d.y + 4*d.z) whenever every component of
+// k - d stays in {0, 1}. The bit mask of those k (in c's numbering): along an axis with d_i = +1 only the upper corners are
+// shared, with d_i = -1 only the lower ones, with d_i = 0 both. A shared vertex has one table entry on every level:
+// the hash and the dense wrap and clamp are functions of the vertex alone (grid_corner_indices).
+__device__ __forceinline__ uint32_t grid_shared_corners(int dx, int dy, int dz) {
+    const uint32_t mx = dx > 0 ? 0xAAu : dx < 0 ? 0x55u : 0xFFu;
+    const uint32_t my = dy > 0 ? 0xCCu : dy < 0 ? 0x33u : 0xFFu;
+    const uint32_t mz = dz > 0 ? 0xF0u : dz < 0 ? 0x0Fu : 0xFFu;
+    return mx & my & mz;
+}
+
+__device__ __forceinline__ bool grid_cells_adjacent(int dx, int dy, int dz) {
+    return (unsigned)(dx + 1) <= 2u && (unsigned)(dy + 1) <= 2u && (unsigned)(dz + 1) <= 2u;
 }
 
 // Scatter of one (sample, level) gradient into the fp32 gradient table: 8 vector reductions of 8 B.

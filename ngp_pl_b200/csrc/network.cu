@@ -843,6 +843,9 @@ k_ngp_bwd3(const NgpNet net, const NgpSamples smp, const float* __restrict__ dL_
 // level. Consecutive samples of a ray fall into the same cell at the coarse levels, so equal cells are
 // contiguous lane runs: their 16 corner contributions are summed with a segmented shuffle reduction and
 // only the head of each run issues the 8 vector reductions (fewer, and far less contended, L2 atomics).
+// At the finer levels a run's next cell is mostly the neighbour across a face, an edge or a vertex, whose shared corners
+// are the same grid vertices and so the same table entries: a head hands those sums to the next head through shared
+// memory instead of issuing them (tests/test_scatter_merge_algorithm_cpu.py replays the rule lane by lane).
 //
 // Level-major order: a work item is a chunk of SCATTER_THREADS consecutive samples x a group of SCATTER_GROUP
 // levels, and the tickets of the device counter hand out every chunk of one group before the next group. So
@@ -859,6 +862,9 @@ __global__ void __launch_bounds__(SCATTER_THREADS, SCATTER_MIN_BLOCKS)
 k_grid_scatter_merged(const NgpNet net, const NgpSamples smp, const uint32_t* __restrict__ dfeat, const int64_t dfeat_stride,
                       const float* __restrict__ loss_scale, float* __restrict__ grad_table, int* __restrict__ sched) {
     __shared__ int s_item[2];
+    // corners handed from a run head to the next (float2 per corner, indexed by the receiving lane; 9 slots per lane
+    // spread the lanes over the banks)
+    __shared__ float2 s_hand[SCATTER_THREADS / 32][32][9];
     const int lane = threadIdx.x & 31;
     const int64_t n = bwd_count(smp);
     const int n_levels = net.meta.n_levels;
@@ -925,9 +931,18 @@ k_grid_scatter_merged(const NgpNet net, const NgpSamples smp, const uint32_t* __
             const bool pvalid = lane > 0 && ((vmask >> (lane - 1)) & 1u);
             const bool head = lane == 0 || !valid || !pvalid || px != c.gx || py != c.gy || pz != c.gz;
             const unsigned heads = __ballot_sync(0xffffffffu, head);
+            const unsigned later = lane == 31 ? 0u : (heads >> (lane + 1));
+            const int run_end = later ? lane + __ffs(later) - 1 : 31;
+            // A valid head whose previous lane is valid starts a run right after another run, whose cell is px, py, pz.
+            // If the two cells are adjacent, its link holds the corners they share (bits 0-7, in this cell's numbering)
+            // and 8 + o, where corner k of the previous cell is corner k + o here (bits 8-11). 0: no link.
+            uint32_t link = 0u;
+            if (valid && pvalid && head) {
+                const int ox = (int)(px - c.gx), oy = (int)(py - c.gy), oz = (int)(pz - c.gz);
+                if (grid_cells_adjacent(ox, oy, oz))
+                    link = grid_shared_corners(ox, oy, oz) | (uint32_t)(ox + 2 * oy + 4 * oz + 8) << 8;
+            }
             if (heads != 0xffffffffu) {
-                const unsigned later = lane == 31 ? 0u : (heads >> (lane + 1));
-                const int run_end = later ? lane + __ffs(later) - 1 : 31;
                 // longest run in the warp bounds the depth of the segmented reduction (warp-uniform)
                 unsigned cont = ~heads;  // bit i set: lane i continues the run of lane i-1
                 int max_run = 1;
@@ -944,12 +959,40 @@ k_grid_scatter_merged(const NgpNet net, const NgpSamples smp, const uint32_t* __
                     }
                 }
             }
+            // Corners shared with the next run's cell, in one pass. A head hands the corners it shares with the next head's
+            // cell to that head, except those it shares with the previous head's cell too: it may receive those, so it
+            // issues them itself. A corner handed over is one the receiver issues (never one it hands on), so every
+            // contribution reaches memory once, after at most one hop.
+            const uint32_t nlink = __shfl_sync(0xffffffffu, link, (run_end + 1) & 31);  // lane 0 has no link
+            uint32_t fwd = 0u, fwd_out = 0u;  // corners handed over, in this cell's and in the next cell's numbering
+            if (valid && head && nlink) {
+                const int o = (int)(nlink >> 8) - 8;  // corner k here is corner k + o of the next cell
+                const uint32_t mine = link & 0xFFu;
+                fwd_out = nlink & 0xFFu & ~(o >= 0 ? mine << o : mine >> -o);
+                fwd = o >= 0 ? fwd_out >> o : fwd_out << -o;
+                float2* dst = s_hand[threadIdx.x >> 5][run_end + 1];
+#pragma unroll
+                for (int k = 0; k < 8; ++k)
+                    if ((fwd >> k) & 1u) dst[k + o] = make_float2(acc[2 * k], acc[2 * k + 1]);
+            }
+            const int phead = lane == 0 ? 0 : 31 - __clz(heads & ((1u << lane) - 1u));
+            const uint32_t recv = __shfl_sync(0xffffffffu, fwd_out, phead);  // what the previous head handed over
+            __syncwarp();
             if (valid && head) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k)
+                    if (link && ((recv >> k) & 1u)) {
+                        const float2 t = s_hand[threadIdx.x >> 5][lane][k];
+                        acc[2 * k] += t.x;
+                        acc[2 * k + 1] += t.y;
+                    }
                 uint32_t idx[8];
                 grid_corner_indices(c, res, entries, hashed, idx);
                 const float* lvl = grad_table + 2 * (size_t)off;
-                grid_scatter_cell_paired(lvl, idx, acc);  // 16-byte reductions for aligned x-corner pairs, 8-byte otherwise
+                // 16-byte reductions for aligned x-corner pairs this head issues both of, 8-byte otherwise
+                grid_scatter_cell_owned(lvl, idx, acc, 0xFFu & ~fwd);
             }
+            __syncwarp();  // read before the next level's hand-over writes
         }
         __syncthreads();
         item = s_item[(it + 1) & 1];
