@@ -20,7 +20,7 @@ extern "C" {
 #endif
 
 #define NGP_MAX_LEVELS 16
-#define NGP_ABI_VERSION 14
+#define NGP_ABI_VERSION 15
 
 int ngp_abi_version(void); /* == NGP_ABI_VERSION of the header the caller was built against */
 
@@ -927,6 +927,97 @@ int ngp_tsdf_mc_count(const float* tsdf, const int32_t* weight, const NgpLattice
 int ngp_tsdf_mc_emit(const float* tsdf, const int32_t* weight, const float* color, const int32_t* color_weight,
                      const NgpLattice* lat, float* vertices, float* normals, uint8_t* colors, int64_t* triangles,
                      int64_t max_vertices, int64_t max_triangles, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ----------------------------------------------------------------------------------------------
+ * Gaussian-splat export: 3D Gaussians in the layout of 3DGS's point_cloud.ply (Kerbl et al. 2023), one per point of the
+ * point-cloud export (stages 1-7 above), with SH colours fitted to the model's radiance, and a forward splat rasteriser
+ * with the 3DGS reference rasteriser's rules. numpy restatement: oracle/splats_ref.py (float64). Positions, normals and
+ * directions are in the model's frame, as the mesh and point exports write them.
+ *
+ * A splat is NGP_SPLAT_FLOATS fp32, in 3DGS's construct_list_of_attributes order: x y z, nx ny nz (the point's normal;
+ * 3DGS writes zeros), f_dc_0..2, f_rest_0..44, opacity, scale_0..2, rot_0..3 (w x y z). f_rest is channel-major:
+ * f_rest[15 c + k - 1] is coefficient k = 1..15 of channel c. Opacity is stored as logit(alpha), scales as log(s).
+ * SH basis (3DGS's sh_utils.py): C0 = 0.28209479177387814; degree 1: -C1 y, C1 z, -C1 x with C1 = 0.4886025119029199;
+ * degree 2: C2_0 xy, C2_1 yz, C2_2 (2zz - xx - yy), C2_3 xz, C2_4 (xx - yy) with C2 = {1.0925484305920792,
+ * -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396}; degree 3: C3_0 y (3xx - yy),
+ * C3_1 xyz, C3_2 y (4zz - xx - yy), C3_3 z (2zz - 3xx - 3yy), C3_4 x (4zz - xx - yy), C3_5 z (xx - yy),
+ * C3_6 x (xx - 3yy) with C3 = {-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154,
+ * -0.4570457994644658, 1.445305721320277, -0.5900435899266435}. A splat's colour seen along the unit direction u is
+ * max(0, sum_k a_k Y_k(u) + 0.5) per channel.
+ *
+ * Stages, per point p with normal n (0 when normals are left out):
+ *   1. Colours over directions: D directions d_j (NGP_SPLAT_MIN_DIRS..NGP_SPLAT_MAX_DIRS; the host computes a Fibonacci
+ *      sphere z_j = 1 - (2j + 1) / D, phi_j = j pi (3 - sqrt 5) in double and rounds it to fp32). sigma(p) and the fp16
+ *      geometric feature h(p) come from ngp_net_forward (density only); then the colour MLP runs on [SH16(d_j) | h(p)]
+ *      through the network core's colour chain. c(p, d_j) is bitwise the rgb ngp_net_forward returns for (p, d_j), and
+ *      is stored as that fp16 value (exact).
+ *   2. SH fit of degree L in 0..3, n_b = (L + 1)^2 basis functions, basis table Y (D, 16) double evaluated at the fp32
+ *      d_j: w_j = max(0, -((d_jx n_x + d_jy n_y) + d_jz n_z)) in double when n != 0, else 1. In double:
+ *      (sum_j w_j y_j y_j^T + ridge (sum_j w_j) I) a_c = sum_j w_j y_j (c_c(p, d_j) - 0.5) over the leading n_b x n_b
+ *      block, by Cholesky, one matrix for the three channels; the sums run over j in order. Coefficients above degree L
+ *      are 0, and all of them are 0 when a pivot of the (right-looking) factorisation is at most NGP_SPLAT_PIVOT_RTOL times
+ *      the largest diagonal entry of the block: a rank-deficient system, e.g. ridge 0 with fewer than n_b directions in
+ *      the hemisphere. Equal to the restatement within 1e-6 relative (the
+ *      sums' order and the solver's differ; the ridge keeps the system conditioned).
+ *   3. Geometry (no contraction, each double operation rounded as numpy's): m = the left-to-right double sum of the
+ *      first min(k, 3) squared neighbour distances of ngp_points_knn over min(k, 3) (0 for k = 0), s = sqrt(max(m,
+ *      1e-7)). NGP_SPLAT_SPHERE, or n = 0: scales (s, s, s), rotation (1, 0, 0, 0). NGP_SPLAT_DISC: u = n / |n|,
+ *      scales (s, s, flatness s) and rotation (1 + u_z, -u_y, u_x, 0) / its norm, the shortest arc taking +z to u, or
+ *      (0, 1, 0, 0) when that norm is 0 (u = -z). alpha = clamp(1 - exp(-sigma 2 s), 0.01, 0.99). The rotation is the
+ *      restatement's bit for bit; log(s), log(flatness s) and logit(alpha) come from the device's double log / exp and
+ *      are within one fp32 ulp of it.
+ * No float atomics: two calls are bitwise equal.
+ *
+ * ngp_splat_colors: sigma (n) fp32, h (n, 16) fp16 scratch, rgb (n, D, 3) fp16 for points (n, 3) and dirs (D, 3) fp32.
+ * ngp_splat_fit: stage 2 from rgb as ngp_splat_colors writes it and basis (D, 16) double; normals may be NULL; writes
+ * f_dc and f_rest of splats (n, NGP_SPLAT_FLOATS) and nothing else. ngp_splat_geometry: stage 3 from dist2 (n, k) of
+ * ngp_points_knn (k in 0..NGP_POINTS_MAX_K) and sigma; normals may be NULL; writes every other field of splats.
+ * No read-back in either. NGP_EINVAL for n outside [0, 2^31), D or L out of range, a negative or non-finite ridge, a
+ * flatness not positive and finite, an unknown shape or a NULL pointer that is needed.
+ *
+ * Rasteriser (ngp_splat_render), forward only, after the 3DGS reference rasteriser:
+ *   - view (device, NGP_SPLAT_VIEW_FLOATS fp32): the c2w pose (3 x 4, R | o, OpenCV axes: x right, y down, z forward),
+ *     fx, fy, cx, cy (pixel centres at i + 0.5, as the loaders' ray directions have them), bg (3).
+ *   - Per splat, fp32: camera point c = R^T (p - o), culled unless c_z > 0.2. Sigma = R_q diag(s^2) R_q^T with R_q from
+ *     the normalised quaternion and s = exp(scale). EWA: t_x = clamp(c_x / c_z, +-1.3 W / (2 fx)) c_z (y likewise with
+ *     H, fy), J = [[fx / c_z, 0, -fx t_x / c_z^2], [0, fy / c_z, -fy t_y / c_z^2]], Sigma2D = J R^T Sigma R J^T + 0.3 I;
+ *     culled unless det > 0. Radius ceil(3 sqrt(lambda_max)) with lambda = mid +- sqrt(max(0.1, mid^2 - det)). Centre
+ *     (fx c_x / c_z + cx - 0.5, fy c_y / c_z + cy - 0.5) in pixel-centre coordinates. Tiles of NGP_SPLAT_TILE^2 pixels:
+ *     the rectangle [(int)((x - r) / 16), (int)((x + r + 15) / 16)) per axis clamped to the grid; culled when empty.
+ *     Colour at u = normalise(p - o) as above; opacity sigmoid(logit).
+ *   - Keys (tile << 32 | depth bits), one per touched tile, radix-sorted (stable: ties keep splat order), then per-tile
+ *     ranges. Per pixel, front to back: power = -(a dx^2 + c dy^2) / 2 - b dx dy with d = centre - pixel; skipped when
+ *     power > 0; alpha = min(0.99, o exp(power)), skipped below 1/255; stop when T (1 - alpha) < 1e-4; C += c alpha T.
+ *     rgb = C + T bg (H W, 3) and opacity = 1 - T (H W), fp32.
+ *   - At most `capacity` keys are sorted: the call reads nothing back. The number of keys the view needs goes to the
+ *     device int64 *n_keys; when it exceeds capacity the image is incomplete and the caller renders again with a
+ *     larger one. So one call with fixed sizes can be captured in a CUDA graph and replayed for any view.
+ * ngp_splat_render_workspace(n, W, H, capacity) is about 64 n + 24 capacity bytes plus cub's temporary storage; 0 (and
+ * NGP_EINVAL from the render) for n outside [0, 2^31), W or H outside 1..NGP_SPLAT_MAX_SIDE or capacity outside
+ * [1, 2^31); the workspace must be 256-B aligned. */
+#define NGP_SPLAT_FLOATS 62
+#define NGP_SPLAT_F_DC 6
+#define NGP_SPLAT_F_REST 9
+#define NGP_SPLAT_OPACITY 54
+#define NGP_SPLAT_SCALE 55
+#define NGP_SPLAT_ROT 58
+#define NGP_SPLAT_MIN_DIRS 16
+#define NGP_SPLAT_MAX_DIRS 1024
+#define NGP_SPLAT_SPHERE 0
+#define NGP_SPLAT_DISC 1
+#define NGP_SPLAT_VIEW_FLOATS 19
+#define NGP_SPLAT_TILE 16
+#define NGP_SPLAT_MAX_SIDE 16384
+#define NGP_SPLAT_PIVOT_RTOL 1e-10
+int ngp_splat_colors(const NgpNet* net, const float* points, int64_t n_points, const float* dirs, int n_dirs, float* sigma,
+                     uint16_t* h, uint16_t* rgb, void* stream);
+int ngp_splat_fit(const uint16_t* rgb, int64_t n_points, int n_dirs, const float* dirs, const double* basis,
+                  const float* normals, int degree, double ridge, float* splats, void* stream);
+int ngp_splat_geometry(const float* points, const float* normals, const float* sigma, const double* dist2, int k,
+                       int64_t n_points, int shape, float flatness, float* splats, void* stream);
+size_t ngp_splat_render_workspace(int64_t n_splats, int W, int H, int64_t capacity);
+int ngp_splat_render(const float* splats, int64_t n_splats, const float* view, int W, int H, int64_t capacity, float* rgb,
+                     float* opacity, int64_t* n_keys, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ----------------------------------------------------------------------------------------------
  * Connected components (numpy + scipy restatement: oracle/components_ref.py), to remove floaters from the occupancy

@@ -9,7 +9,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 14  #NGP_ABI_VERSION in include/ngp_b200.h
+ABI_VERSION = 15  #NGP_ABI_VERSION in include/ngp_b200.h
 
 NGP_MAX_LEVELS = 16
 NGP_DENSITY_MLP_PARAMS = 3072
@@ -28,6 +28,14 @@ NGP_TEXTURE_CHUNK_SAMPLES = 1 << 22
 NGP_POINTS_MAX_K = 64
 NGP_POINTS_KNN_MAX_CELLS = 1 << 22
 NGP_TSDF_GROUP = 64
+NGP_SPLAT_FLOATS = 62
+NGP_SPLAT_MIN_DIRS = 16
+NGP_SPLAT_MAX_DIRS = 1024
+NGP_SPLAT_SPHERE = 0
+NGP_SPLAT_DISC = 1
+NGP_SPLAT_VIEW_FLOATS = 19
+NGP_SPLAT_MAX_SIDE = 16384
+NGP_SPLAT_PIVOT_RTOL = 1e-10
 NGP_VIEW_IMAGES_WORKSPACE = 4096
 NGP_PNG_FIXED = 0
 NGP_PNG_DYNAMIC = 1
@@ -252,6 +260,11 @@ SIGNATURES = {
     "ngp_tsdf_mc_workspace": (_sz, [C.POINTER(NgpLattice)]),
     "ngp_tsdf_mc_count": (_i, [_P, _P, C.POINTER(NgpLattice), _P, _P, _sz, _P]),
     "ngp_tsdf_mc_emit": (_i, [_P, _P, _P, _P, C.POINTER(NgpLattice), _P, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
+    "ngp_splat_colors": (_i, [C.POINTER(NgpNet), _P, _i64, _P, _i, _P, _P, _P, _P]),
+    "ngp_splat_fit": (_i, [_P, _i64, _i, _P, _P, _P, _i, C.c_double, _P, _P]),
+    "ngp_splat_geometry": (_i, [_P, _P, _P, _P, _i, _i64, _i, _f, _P, _P]),
+    "ngp_splat_render_workspace": (_sz, [_i64, _i, _i, _i64]),
+    "ngp_splat_render": (_i, [_P, _i64, _P, _i, _i, _i64, _P, _P, _P, _P, _sz, _P]),
     "ngp_grid_components": (_i, [_P, _i, _i, _f, _P, _P, _P]),
     "ngp_grid_components_clean": (_i, [_P, _P, _i, _i, _f, _P, _P, _P, _P, _P]),
     "ngp_components_select_workspace": (_sz, [_i64]),

@@ -16,7 +16,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libngp_b200.so")
 
 SOURCES = ["vren_ops.cu", "network.cu", "train.cu", "infer.cu", "modules.cu", "metrics.cu", "mesh.cu", "lpips.cu", "stage.cu", "images.cu", "jpeg.cu",
-           "texture.cu", "points.cu", "components.cu", "fusion.cu"]
+           "texture.cu", "points.cu", "components.cu", "fusion.cu", "splats.cu"]
 # texture.cu's, points.cu's and fusion.cu's arithmetic must round operation by operation as their numpy restatements
 # (oracle/mesh_texture.py, oracle/points_ref.py, oracle/tsdf_ref.py) do
 SOURCE_FLAGS = {"texture.cu": ["-fmad=false"], "points.cu": ["-fmad=false"], "fusion.cu": ["-fmad=false"]}
