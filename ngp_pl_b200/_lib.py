@@ -1,289 +1,161 @@
 """ctypes binding of libngp_b200.so (the C-ABI declared in include/ngp_b200.h).
 
+The binding is read from the header itself at import, so it cannot drift from what the library was compiled against:
+every valued `#define NGP_*` becomes a module constant, every `typedef struct { ... } Ngp*;` a ctypes.Structure of the
+same name, and every function declaration an entry of SIGNATURES (name -> (restype, argtypes)). A declaration outside
+the rules parse_header states is an import error, never a guess.
+
 There is NO fallback: if the library is missing or a symbol is absent this module raises, and every
 operator built on it raises with it. (The CPU oracle under /oracle is test infrastructure and is never
 imported from here.)
 """
+import ast
 import ctypes as C
+import operator
 import os
+import re
+
+from .build import HEADER
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libngp_b200.so")
-ABI_VERSION = 15  #NGP_ABI_VERSION in include/ngp_b200.h
 
-NGP_MAX_LEVELS = 16
-NGP_DENSITY_MLP_PARAMS = 3072
-NGP_RGB_MLP_PARAMS = 7168
-NGP_MC_SLAB_POINTS = 1 << 20
-NGP_MESH_BRICK = 8
-NGP_MESH_MAX_N = 8192
-NGP_MESH_CHUNK_BRICKS = 1 << 16
-NGP_SIMPLIFY_MAX_GRID = 65536
-NGP_TEXTURE_MIN_SIZE = 16
-NGP_TEXTURE_MAX_SIZE = 16384
-NGP_TEXTURE_MIN_SQUARE = 4
-NGP_TEXTURE_MARGIN = 1
-NGP_TEXTURE_MAX_SAMPLES = 256
-NGP_TEXTURE_CHUNK_SAMPLES = 1 << 22
-NGP_POINTS_MAX_K = 64
-NGP_POINTS_KNN_MAX_CELLS = 1 << 22
-NGP_TSDF_GROUP = 64
-NGP_SPLAT_FLOATS = 62
-NGP_SPLAT_MIN_DIRS = 16
-NGP_SPLAT_MAX_DIRS = 1024
-NGP_SPLAT_SPHERE = 0
-NGP_SPLAT_DISC = 1
-NGP_SPLAT_VIEW_FLOATS = 19
-NGP_SPLAT_MAX_SIDE = 16384
-NGP_SPLAT_PIVOT_RTOL = 1e-10
-NGP_VIEW_IMAGES_WORKSPACE = 4096
-NGP_PNG_FIXED = 0
-NGP_PNG_DYNAMIC = 1
-# ngp_render_infer_layout's fields, in the order of NGP_INFER_T_CUR .. NGP_INFER_COUNTERS
-NGP_INFER_FIELDS = ("t_cur", "t_end", "alive0", "alive1", "ray_start", "ray_n", "ray_idx", "ts", "deltas", "sigmas",
-                    "rgbs", "counters")
-NGP_INFER_STATE_OFFSET = 32
-NGP_INFER_TOTAL_OFFSET = 64
+# C scalar types by value, in parameters, return types and struct fields; any pointer is c_void_p, except a function
+# parameter that points to an Ngp* struct, which is POINTER(struct)
+_SCALARS = {"int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint32_t": C.c_uint32, "uint64_t": C.c_uint64,
+            "float": C.c_float, "double": C.c_double, "size_t": C.c_size_t, "unsigned long long": C.c_ulonglong}
+_OPS = {ast.Add: operator.add, ast.LShift: operator.lshift}
+# `type name`, `type* name` or `type name[dim]`
+_DECLARATOR = re.compile(r"\s*([\w\s]*\w)(?:\s*(\*+)\s*|\s+)(\w+)\s*(?:\[([^\]]*)\])?\s*")
+# the further declarators of a comma list: `name`, `*name` or `name[dim]`
+_MORE = re.compile(r"\s*(\*+)?\s*(\w+)\s*(?:\[([^\]]*)\])?\s*")
+_STATEMENT = re.compile(r"\s*(?:typedef\s+struct\s*\{([^{}]*)\}\s*(\w+)|([^;{}]+?))\s*;")
 
 
-class NgpGridMeta(C.Structure):
-    _fields_ = [
-        ("n_levels", C.c_int32),
-        ("hashed_mask", C.c_uint32),
-        ("offset", C.c_uint32 * (NGP_MAX_LEVELS + 1)),
-        ("res", C.c_uint32 * NGP_MAX_LEVELS),
-        ("scale", C.c_float * NGP_MAX_LEVELS),
-    ]
+def _fail(what, why):
+    raise RuntimeError("%s: %s" % (what, why))
 
 
-class NgpNet(C.Structure):
-    _fields_ = [
-        ("enc_params_h", C.c_void_p),
-        ("rgb_params_h", C.c_void_p),
-        ("meta", NgpGridMeta),
-        ("xyz_min", C.c_float * 3),
-        ("xyz_max", C.c_float * 3),
-        ("rgb_act", C.c_int32),
-    ]
+def _constant(text, consts, what):
+    """value of a #define or array size: integer and float literals, earlier NGP_* names, `+`, `<<` and parentheses"""
+    def ev(node):
+        if isinstance(node, ast.Constant) and type(node.value) in (int, float):
+            return node.value
+        if isinstance(node, ast.Name) and node.id in consts:
+            return consts[node.id]
+        if isinstance(node, ast.BinOp) and type(node.op) in _OPS:
+            return _OPS[type(node.op)](ev(node.left), ev(node.right))
+        raise ValueError
+    try:
+        return ev(ast.parse(text.strip(), mode="eval").body)
+    except (SyntaxError, ValueError, TypeError):
+        _fail(what, "cannot evaluate %r" % text.strip())
 
 
-class NgpSamples(C.Structure):
-    _fields_ = [
-        ("xyzs", C.c_void_p),
-        ("dirs", C.c_void_p),
-        ("rays_o", C.c_void_p),
-        ("rays_d", C.c_void_p),
-        ("ray_idx", C.c_void_p),
-        ("ts", C.c_void_p),
-        ("n", C.c_int64),
-        ("n_dev", C.c_void_p),
-        ("live_idx", C.c_void_p),
-        ("n_live_dev", C.c_void_p),
-    ]
+def _ctype(base, stars, structs, what, struct_pointers):
+    base = " ".join(w for w in base.split() if w != "const")
+    if stars:
+        return C.POINTER(structs[base]) if struct_pointers and base in structs else C.c_void_p
+    if base in _SCALARS:
+        return _SCALARS[base]
+    if base in structs:
+        return structs[base]
+    _fail(what, "unsupported type %r" % base)
 
 
-class NgpLattice(C.Structure):
-    """Mirror of NgpLattice in include/ngp_b200.h."""
-    _fields_ = [
-        ("n", C.c_int32 * 3),
-        ("lo", C.c_float * 3),
-        ("step", C.c_float * 3),
-    ]
+def _fields(body, structs, consts, name):
+    fields = []
+    for decl in filter(str.strip, body.split(";")):
+        first, *more = decl.split(",")
+        m = _DECLARATOR.fullmatch(first)
+        if m is None or not all(_MORE.fullmatch(d) for d in more):
+            _fail(name, "cannot read the field %r" % " ".join(decl.split()))
+        base = m.group(1)
+        for stars, field, dim in [m.groups()[1:]] + [_MORE.fullmatch(d).groups() for d in more]:
+            what = "%s.%s" % (name, field)
+            t = _ctype(base, stars, structs, what, False)
+            if dim is not None:
+                n = _constant(dim, consts, what)
+                if type(n) is not int or n < 1:
+                    _fail(what, "array size %r is not a positive integer" % dim)
+                t = t * n
+            fields.append((field, t))
+    return fields
 
 
-class NgpClusterGrid(C.Structure):
-    """Mirror of NgpClusterGrid in include/ngp_b200.h."""
-    _fields_ = [
-        ("lo", C.c_float * 3),
-        ("h", C.c_float),
-        ("n", C.c_int32 * 3),
-    ]
+def _function(decl, structs):
+    m = re.fullmatch(r"(.*?)\((.*)\)", decl, re.S)
+    head = m and _DECLARATOR.fullmatch(m.group(1))
+    if not head or head.group(4) is not None:
+        _fail(repr(" ".join(decl.split())), "not a function declaration")
+    base, stars, name, _ = head.groups()
+    args = []
+    if m.group(2).strip() != "void":
+        for p in m.group(2).split(","):
+            a = _DECLARATOR.fullmatch(p)
+            if a is None or a.group(4) is not None:
+                _fail(name, "cannot read the parameter %r" % " ".join(p.split()))
+            args.append(_ctype(a.group(1), a.group(2), structs, name, True))
+    return name, (_ctype(base, stars, structs, name, True), args)
 
 
-class NgpTrainCfg(C.Structure):
-    """Mirror of NgpTrainCfg in include/ngp_b200.h."""
-    _fields_ = [
-        ("n_rays", C.c_int32),
-        ("cascades", C.c_int32),
-        ("grid_size", C.c_int32),
-        ("max_samples", C.c_int32),
-        ("scale", C.c_float),
-        ("exp_step_factor", C.c_float),
-        ("T_threshold", C.c_float),
-        ("near_distance", C.c_float),
-        ("center", C.c_float * 3),
-        ("half_size", C.c_float * 3),
-        ("bg", C.c_float * 3),
-        ("lambda_opacity", C.c_float),
-        ("max_total_samples", C.c_int64),
-    ]
+def parse_header(path):
+    """(constants, structs, signatures) of a C header in include/ngp_b200.h's dialect: `#define NGP_* value`
+    (_constant's expressions; a define without a value is skipped), `typedef struct { fields } Ngp*;` (comma lists,
+    arrays of constant size, nested structs by value, pointers as c_void_p) and function declarations over _SCALARS,
+    pointers and `(void)`. RuntimeError naming the declaration for anything else, and naming the path when the file
+    cannot be read."""
+    try:
+        with open(path) as f:
+            src = f.read()
+    except OSError as e:
+        raise RuntimeError("ngp_pl_b200: cannot read the C header %s: %s" % (path, e))
+    try:
+        return _parse(src)
+    except RuntimeError as e:
+        raise RuntimeError("ngp_pl_b200: %s: %s" % (path, e)) from None
 
 
-class NgpInferCfg(C.Structure):
-    """Mirror of NgpInferCfg in include/ngp_b200.h."""
-    _fields_ = [
-        ("n_rays", C.c_int32),
-        ("cascades", C.c_int32),
-        ("grid_size", C.c_int32),
-        ("max_samples", C.c_int32),
-        ("scale", C.c_float),
-        ("exp_step_factor", C.c_float),
-        ("T_threshold", C.c_float),
-        ("near_distance", C.c_float),
-        ("center", C.c_float * 3),
-        ("half_size", C.c_float * 3),
-        ("bg", C.c_float * 3),
-        ("sample_budget", C.c_int32),
-        ("max_round_samples", C.c_int64),
-    ]
+def _parse(src):
+    src = re.sub(r"/\*.*?\*/", " ", src, flags=re.S)
+    src = re.sub(r"//[^\n]*", "", src)
+    src = re.sub(r"^[ \t]*#[ \t]*ifdef[ \t]+__cplusplus\b.*?^[ \t]*#[ \t]*endif\b", "", src, flags=re.S | re.M)  # extern "C"
+    consts = {}
+    for name, value in re.findall(r"^[ \t]*#[ \t]*define[ \t]+(\S+)[ \t]*(.*)$", src, re.M):
+        if not re.fullmatch(r"NGP_\w+", name):
+            _fail("#define " + name, "only NGP_* object-like macros are read")
+        if value.strip():
+            consts[name] = _constant(value, consts, "#define " + name)
+    src = re.sub(r"^[ \t]*#.*$", "", src, flags=re.M)
+    structs, signatures = {}, {}
+    pos, end = 0, len(src.rstrip())
+    while pos < end:
+        m = _STATEMENT.match(src, pos)
+        if m is None:
+            _fail(repr(" ".join(src[pos:].split())[:80]), "not a declaration")
+        pos = m.end()
+        body, name, decl = m.groups()
+        if decl is None:
+            structs[name] = type(name, (C.Structure,), {"_fields_": _fields(body, structs, consts, name),
+                                                        "__module__": __name__,
+                                                        "__doc__": "Mirror of %s in include/ngp_b200.h." % name})
+        else:
+            fn, sig = _function(decl, structs)
+            signatures[fn] = sig
+    return consts, structs, signatures
 
 
-class NgpViewCfg(C.Structure):
-    """Mirror of NgpViewCfg in include/ngp_b200.h."""
-    _fields_ = [
-        ("mode", C.c_int32),
-        ("quality", C.c_int32),
-        ("H", C.c_int32),
-        ("W", C.c_int32),
-    ]
-
-
-class NgpTrainBuffers(C.Structure):
-    """Mirror of NgpTrainBuffers in include/ngp_b200.h."""
-    _fields_ = [(n, C.c_void_p) for n in (
-        "rays_o", "rays_d", "noise", "density_bitfield",
-        "stage_t", "stage_dt", "n_samples", "offsets", "counters", "rgb", "opacity", "depth",
-        "ray_idx", "ts", "deltas", "sigmas", "rgbs", "ws", "dsigmas", "drgbs", "live_idx", "feat_save", "scalars",
-        "scan_temp")] + [("scan_temp_bytes", C.c_size_t), ("bwd_workspace", C.c_void_p), ("bwd_workspace_bytes", C.c_size_t),
-                                  ("bg_dev", C.c_void_p)]
-
-
-_P = C.c_void_p
-_i = C.c_int
-_i64 = C.c_int64
-_f = C.c_float
-_sz = C.c_size_t
-
-# name -> (restype, argtypes). Every symbol include/ngp_b200.h declares must be listed here;
-# tests/test_abi.py checks header <-> table <-> library agreement.
-SIGNATURES = {
-    "ngp_abi_version": (_i, []),
-    "ngp_launch_count": (C.c_ulonglong, []),
-    "ngp_trace_set": (_i, [_P]),
-    "ngp_ray_aabb_intersect": (_i, [_P, _P, _P, _P, _i, _i, _i, _P, _P, _P, _P]),
-    "ngp_ray_sphere_intersect": (_i, [_P, _P, _P, _P, _i, _i, _i, _P, _P, _P, _P]),
-    "ngp_packbits": (_i, [_P, _i, _i64, _f, _P, _P, _P]),
-    "ngp_morton3D": (_i, [_P, _i, _P, _P]),
-    "ngp_morton3D_invert": (_i, [_P, _i, _P, _P]),
-    "ngp_raymarching_train_workspace": (_sz, [_i]),
-    "ngp_raymarching_train_workspace2": (_sz, [_i, _i]),
-    "ngp_raymarching_train": (_i, [_P, _P, _P, _P, _i, _f, _f, _P, _i, _i, _i, _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
-    "ngp_raymarching_test": (_i, [_P, _P, _P, _P, _P, _i, _f, _f, _i, _i, _i, _i, _P, _P, _P, _P, _P, _P]),
-    "ngp_composite_train_fw": (_i, [_P, _P, _P, _P, _P, _f, _i, _i64, _P, _P, _P, _P, _P, _P]),
-    "ngp_composite_train_bw": (_i, [_P] * 13 + [_f, _i, _i64, _P, _P, _P]),
-    "ngp_composite_test_fw": (_i, [_P, _P, _P, _P, _P, _P, _f, _P, _i, _i, _P, _P, _P, _P]),
-    "ngp_distortion_loss_fw": (_i, [_P, _P, _P, _P, _i, _i64, _P, _P, _P, _P]),
-    "ngp_distortion_loss_bw": (_i, [_P, _P, _P, _P, _P, _P, _P, _i, _i64, _P, _P]),
-    "ngp_grid_meta": (C.c_uint32, [_i, _i, _i, _f, C.POINTER(NgpGridMeta)]),
-    "ngp_cast_params": (_i, [_P, _P, _i64, _P]),
-    "ngp_net_forward": (_i, [C.POINTER(NgpNet), C.POINTER(NgpSamples), _i, _P, _P, _P, _P, _P]),
-    "ngp_net_backward_workspace": (_sz, [_i64]),
-    "ngp_net_backward": (_i, [C.POINTER(NgpNet), C.POINTER(NgpSamples), _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
-    "ngp_net_backward_mlp": (_i, [C.POINTER(NgpNet), C.POINTER(NgpSamples), _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
-    "ngp_net_backward_scatter": (_i, [C.POINTER(NgpNet), C.POINTER(NgpSamples), _P, _P, _P, _sz, _P]),
-    "ngp_sh_encode": (_i, [_P, _i64, _P, _P]),
-    "ngp_mlp_rgb_forward": (_i, [_P, _P, _i64, _i, _P, _P]),
-    "ngp_mlp_rgb_backward": (_i, [_P, _P, _P, _i64, _i, _P, _P, _P, _P]),
-    "ngp_enc_backward": (_i, [C.POINTER(NgpNet), C.POINTER(NgpSamples), _P, _P, _P, _P, _P, _sz, _P]),
-    "ngp_grad_scale": (_i, [_P, _P, _P, _i64, _P, _P, _P]),
-    "ngp_train_scan_temp_bytes": (_sz, [_i]),
-    "ngp_render_train_fwd": (_i, [C.POINTER(NgpNet), C.POINTER(NgpTrainCfg), C.POINTER(NgpTrainBuffers), _P]),
-    "ngp_render_train_march": (_i, [C.POINTER(NgpTrainCfg), C.POINTER(NgpTrainBuffers), _P]),
-    "ngp_render_train_net": (_i, [C.POINTER(NgpNet), C.POINTER(NgpTrainCfg), C.POINTER(NgpTrainBuffers), _P]),
-    "ngp_render_train_step": (_i, [C.POINTER(NgpNet), C.POINTER(NgpTrainCfg), C.POINTER(NgpTrainBuffers), _P, _P, _P, _P]),
-    "ngp_render_train_bwd": (_i, [C.POINTER(NgpNet), C.POINTER(NgpTrainCfg), C.POINTER(NgpTrainBuffers),
-                                  _P, _P, _P, _P, _P, _P, _P]),
-    "ngp_nerf_loss_grad": (_i, [C.POINTER(NgpTrainCfg), C.POINTER(NgpTrainBuffers), _P, _P, _P, _P]),
-    "ngp_adam_step": (_i, [_P, _P, _P, _P, _P, _i64, _P, _P, _f, _f, _f, _f, _i, _P]),
-    "ngp_adam_step_p2p": (_i, [_i, _i, _P, _P, _P, _P, _P, _i64, _P, _P, _f, _f, _f, _i, _P]),
-    "ngp_adam_step_fused": (_i, [_i, _i, _P, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P, _i64, _P, _P, _P, _P, _f, _f, _f, _i, _P]),
-    "ngp_train_log_step": (_i, [_P, _P, _P, _P, _P, _i64, _P, _i, _P]),
-    "ngp_gen_rays": (_i, [_P, _P, _P, _P, _P, _i64, _i, _P, _P, _P, _P]),
-    "ngp_sample_rays": (_i, [_P, _P, _P, _i, _i64, _i, C.c_uint32, C.c_uint32, _P, _P, _P, _P, _P, _P]),
-    "ngp_sample_rays_ex": (_i, [_P, _P, _P, _i, _i, _i, _i64, _i, C.c_uint32, C.c_uint32, _P, _P, _P, _P, _P, _P]),
-    "ngp_stage_image": (_i, [_P, _i, _i, _i, _i, _i, _i, _P, _P]),
-    "ngp_render_infer_workspace": (_sz, [_i, _i64]),
-    "ngp_render_infer_layout": (_sz, [_i, _i64, _P]),
-    "ngp_render_infer": (_i, [C.POINTER(NgpNet), C.POINTER(NgpInferCfg), _P, _P, _P, _P, _P, _P, _P, _i, _i, _i, _P,
-                              _P, _sz, _P]),
-    "ngp_render_infer_frame": (_i, [C.POINTER(NgpNet), C.POINTER(NgpInferCfg), _P, _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
-    "ngp_render_view_workspace": (_sz, [C.POINTER(NgpInferCfg), C.POINTER(NgpViewCfg)]),
-    "ngp_render_view_frame": (_i, [C.POINTER(NgpNet), C.POINTER(NgpInferCfg), C.POINTER(NgpViewCfg)] + [_P] * 9 +
-                              [_sz, _P, _P, _sz, _P]),
-    "ngp_update_grid_workspace": (_sz, [_i, _i]),
-    "ngp_update_density_grid": (_i, [C.POINTER(NgpNet), _P, _P, _P, _i, _i, _f, _f, _i, _f, C.c_uint32, _P, _sz, _P]),
-    "ngp_update_density_grid_pick": (_i, [_P, _i, _i, _f, _f, _i, C.c_uint32, _P, _sz, _P]),
-    "ngp_update_density_grid_eval": (_i, [C.POINTER(NgpNet), _P, _P, _P, _i, _i, _f, _i, _f, _P, _sz, _P]),
-    "ngp_image_metrics_workspace": (_sz, [_i, _i]),
-    "ngp_image_metrics": (_i, [_P, _P, _i, _i, _i, _f, _P, _P, _P, _sz, _P]),
-    "ngp_lpips_weights_bytes": (_sz, []),
-    "ngp_lpips_workspace": (_sz, [_i, _i]),
-    "ngp_lpips": (_i, [_P, _P, _P, _i, _i, _i, _P, _P, _sz, _P]),
-    "ngp_density_lattice": (_i, [C.POINTER(NgpNet), C.POINTER(NgpLattice), _P, _P]),
-    "ngp_marching_cubes_workspace": (_sz, [C.POINTER(NgpLattice)]),
-    "ngp_marching_cubes_count": (_i, [_P, C.POINTER(NgpLattice), _f, _P, _P, _sz, _P]),
-    "ngp_marching_cubes_emit": (_i, [_P, C.POINTER(NgpLattice), _f, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
-    "ngp_mesh_bricks_bytes": (_sz, [C.POINTER(NgpLattice)]),
-    "ngp_mesh_brick_mask": (_i, [_P, _i, _i, _f, C.POINTER(NgpLattice), _P, _P]),
-    "ngp_density_bricks": (_i, [C.POINTER(NgpNet), C.POINTER(NgpLattice), _P, _i64, _i, _P, _P, _P]),
-    "ngp_mesh_sparse_workspace": (_sz, [C.POINTER(NgpLattice)]),
-    "ngp_mesh_sparse_bricks": (_i, [C.POINTER(NgpNet), C.POINTER(NgpLattice), _f, _P, _P, _P, _sz, _P]),
-    "ngp_mesh_surface_workspace": (_sz, [C.POINTER(NgpLattice), _i64]),
-    "ngp_mesh_sparse_count": (_i, [C.POINTER(NgpNet), C.POINTER(NgpLattice), _f, _P, _i64, _P, _P, _sz, _P, _sz, _P]),
-    "ngp_mesh_sparse_emit": (_i, [C.POINTER(NgpLattice), _f, _i64, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
-    "ngp_mesh_simplify_workspace": (_sz, [_i64, _i64]),
-    "ngp_mesh_simplify_count": (_i, [_P, _i64, _P, _i64, C.POINTER(NgpClusterGrid), _P, _P, _sz, _P]),
-    "ngp_mesh_simplify_emit": (_i, [_P, _i64, _i64, _P, _P, _P, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
-    "ngp_mesh_texture_workspace": (_sz, [_i64, _i64, _i]),
-    "ngp_mesh_texture_atlas": (_i, [_P, _i64, _P, _i64, _i, _P, _P, _P, _P, _sz, _P]),
-    "ngp_mesh_texture_texels": (_i, [_P, _P, _i64, _P, _i64, _i, _P, _i64, _P, _P, _P, _P, _P, _sz, _P]),
-    "ngp_mesh_texture_bake_workspace": (_sz, [_i]),
-    "ngp_mesh_texture_bake": (_i, [C.POINTER(NgpNet), _i, _i64, _P, _P, _P, _f, _i, _P, _P, _sz, _P]),
-    "ngp_points_workspace": (_sz, [_i64]),
-    "ngp_points_rays": (_i, [_i64, _i64, _i64, _i64, _i, _P, _P, _P, _P, _P, _P, _P]),
-    "ngp_points_backproject": (_i, [_P, _P, _P, _P, _P, _i64, _f, _P, _P, _P, _P, _P, _P, _sz, _P]),
-    "ngp_points_voxel": (_i, [_P, _P, _P, _i64, C.POINTER(NgpClusterGrid), _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
-    "ngp_points_knn": (_i, [_P, _i64, _i, _P, _P, _P, _sz, _P]),
-    "ngp_points_outliers": (_i, [_P, _P, _P, _i64, _i, _P, C.c_double, _P, _P, _P, _P, _P, _P, _P, _sz, _P]),
-    "ngp_points_normals": (_i, [_P, _P, _i64, _i, _P, _P, _P]),
-    "ngp_tsdf_integrate": (_i, [C.POINTER(NgpLattice), _f, _i, _P, _P, _i, _i, _P, _P, _P, _P, _f, _P, _P, _P, _P, _P]),
-    "ngp_tsdf_mc_workspace": (_sz, [C.POINTER(NgpLattice)]),
-    "ngp_tsdf_mc_count": (_i, [_P, _P, C.POINTER(NgpLattice), _P, _P, _sz, _P]),
-    "ngp_tsdf_mc_emit": (_i, [_P, _P, _P, _P, C.POINTER(NgpLattice), _P, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
-    "ngp_splat_colors": (_i, [C.POINTER(NgpNet), _P, _i64, _P, _i, _P, _P, _P, _P]),
-    "ngp_splat_fit": (_i, [_P, _i64, _i, _P, _P, _P, _i, C.c_double, _P, _P]),
-    "ngp_splat_geometry": (_i, [_P, _P, _P, _P, _i, _i64, _i, _f, _P, _P]),
-    "ngp_splat_render_workspace": (_sz, [_i64, _i, _i, _i64]),
-    "ngp_splat_render": (_i, [_P, _i64, _P, _i, _i, _i64, _P, _P, _P, _P, _sz, _P]),
-    "ngp_grid_components": (_i, [_P, _i, _i, _f, _P, _P, _P]),
-    "ngp_grid_components_clean": (_i, [_P, _P, _i, _i, _f, _P, _P, _P, _P, _P]),
-    "ngp_components_select_workspace": (_sz, [_i64]),
-    "ngp_components_select": (_i, [_P, _P, _i64, _i64, _i64, _P, _P, _P, _sz, _P]),
-    "ngp_mesh_components_workspace": (_sz, [_i64, _i64]),
-    "ngp_mesh_components": (_i, [_P, _i64, _i64, _P, _P, _P, _sz, _P]),
-    "ngp_mesh_filter_workspace": (_sz, [_i64, _i64]),
-    "ngp_mesh_filter_count": (_i, [_P, _i64, _i64, _P, _P, _P, _P, _sz, _P]),
-    "ngp_mesh_filter_emit": (_i, [_P, _P, _P, _P, _i64, _i64, _P, _P, _P, _P, _i64, _i64, _P, _sz, _P]),
-    "ngp_view_images": (_i, [_P, _P, _i, _i, _P, _P, _P, _sz, _P]),
-    "ngp_png_workspace": (_sz, [_i, _i]),
-    "ngp_png_capacity": (_sz, [_i, _i]),
-    "ngp_png_encode": (_i, [_P, _i, _i, _P, _sz, _P, _P, _sz, _P]),
-    "ngp_png_workspace_mode": (_sz, [_i, _i, _i]),
-    "ngp_png_encode_mode": (_i, [_P, _i, _i, _i, _P, _sz, _P, _P, _sz, _P]),
-    "ngp_jpeg_workspace": (_sz, [_i, _i]),
-    "ngp_jpeg_capacity": (_sz, [_i, _i]),
-    "ngp_jpeg_encode": (_i, [_P, _i, _i, _i, _P, _sz, _P, _P, _sz, _P]),
-}
+_consts, _structs, SIGNATURES = parse_header(HEADER)
+globals().update(_consts)
+globals().update(_structs)
+ABI_VERSION = _consts["NGP_ABI_VERSION"]
+# ngp_render_infer_layout's fields: the NGP_INFER_* indices 0 .. NGP_INFER_LAYOUT_FIELDS - 1, lower-cased, in order
+_n_infer = _consts["NGP_INFER_LAYOUT_FIELDS"]
+_infer = sorted((v, n[len("NGP_INFER_"):].lower()) for n, v in _consts.items()
+                if n.startswith("NGP_INFER_") and 0 <= v < _n_infer)
+if [v for v, _ in _infer] != list(range(_n_infer)):
+    raise RuntimeError("ngp_pl_b200: %s: the NGP_INFER_* field indices are not 0 .. NGP_INFER_LAYOUT_FIELDS - 1" % HEADER)
+NGP_INFER_FIELDS = tuple(n for _, n in _infer)
 
 _lib = None
 
@@ -322,7 +194,7 @@ def infer_layout(n_rays, max_round_samples):
 
 
 def grid_meta(n_levels, log2_hashmap_size, base_resolution, per_level_scale):
-    m = NgpGridMeta()
+    m = _structs["NgpGridMeta"]()
     total = lib().ngp_grid_meta(int(n_levels), int(log2_hashmap_size), int(base_resolution),
                                 float(per_level_scale), C.byref(m))
     if total == 0:

@@ -12,6 +12,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
+HEADER = os.path.join(INCLUDE, "ngp_b200.h")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libngp_b200.so")
 
@@ -42,8 +43,7 @@ def sources():
 
 def build(force=False, verbose=False):
     srcs = sources()
-    deps = srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")] + \
-           [os.path.join(INCLUDE, "ngp_b200.h")]
+    deps = srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")] + [HEADER]
     stamp = os.path.join(OBJ, "stamp")
     dg = _digest(deps)
     if not force and os.path.exists(LIB) and os.path.exists(stamp) and open(stamp).read() == dg:

@@ -26,30 +26,19 @@ import numpy as np
 import torch
 
 from . import _lib
-from .mesh import _chk, _need, _st, _three, lattice
-from .models.networks import _net_struct
-from .models.rendering import MAX_SAMPLES, NEAR_DISTANCE
-from .points import CHUNK, MAX_RAYS
+from .mesh import _chk, _need, _np, _st, _three, lattice
+from .models.rendering import default_exp_step_factor, infer_cfg
+from .points import CHUNK, MAX_RAYS, _render_chunks
 
 STATE_BYTES = 24   # per lattice point: tsdf, weight, colour mean (3), colour weight
 MAP_BYTES = 20     # per rendered pixel: opacity, depth, rgb
 
 
-def _np(a):
-    return a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
-
-
 def _infer_cfg(model, B, exp_step_factor):
-    cfg = _lib.NgpInferCfg()
-    cfg.n_rays, cfg.cascades, cfg.grid_size, cfg.max_samples = B, model.cascades, model.grid_size, MAX_SAMPLES
-    cfg.scale, cfg.exp_step_factor = float(model.scale), float(exp_step_factor)
-    cfg.T_threshold, cfg.near_distance = 1e-4, NEAR_DISTANCE
-    c, h = model.center.flatten().tolist(), model.half_size.flatten().tolist()
-    for k in range(3):
-        cfg.center[k], cfg.half_size[k], cfg.bg[k] = c[k], h[k], 0.0
-    cfg.sample_budget = MAX_SAMPLES
-    cfg.max_round_samples = max(4 * B, 1 << 16)
-    return cfg, c, h
+    """render_views' configuration for chunks of B rays (the point-cloud export's: black background, T_threshold 1e-4,
+    MAX_SAMPLES), with the model's box centre and half size, behind which the spare rays of a short chunk start"""
+    return (infer_cfg(model, B, exp_step_factor, 0.0), model.center.flatten().tolist(),
+            model.half_size.flatten().tolist())
 
 
 @torch.no_grad()
@@ -67,38 +56,21 @@ def render_views(model, poses, directions, chunk=CHUNK, exp_step_factor=None):
     if V < 1 or HW < 1:
         raise RuntimeError("ngp_pl_b200.fusion.render_views: no cameras (%d poses, %d directions)" % (V, HW))
     if exp_step_factor is None:
-        exp_step_factor = 1 / 256 if float(model.scale) > 0.5 else 0.0
+        exp_step_factor = default_exp_step_factor(model)
     N = V * HW
     B = min(int(chunk), N)
     n_chunks = (N + B - 1) // B
-    cfg, c, h = _infer_cfg(model, B, exp_step_factor)
-    L = _lib.lib()
+    cfg = _infer_cfg(model, B, exp_step_factor)[0]
     with torch.cuda.device(dev):
-        infer_bytes = L.ngp_render_infer_workspace(B, cfg.max_round_samples)
+        infer_bytes = _lib.lib().ngp_render_infer_workspace(B, cfg.max_round_samples)
         # the maps are padded to whole chunks, so every chunk renders straight into them
         _need(dev, n_chunks * B * MAP_BYTES + B * 40 + infer_bytes, "the maps of %d views of %d pixels" % (V, HW),
               "render_views")
-        ws = torch.empty(infer_bytes, device=dev, dtype=torch.uint8)
-        idx = torch.empty(2, B, device=dev, dtype=torch.int64)
-        o, d = torch.empty(B, 3, device=dev), torch.empty(B, 3, device=dev)
         opacity = torch.empty(n_chunks * B, device=dev)
         depth = torch.empty(n_chunks * B, device=dev)
         rgb = torch.empty(n_chunks * B, 3, device=dev)
-        total = torch.zeros(1, device=dev, dtype=torch.int64)
-        net, keep = _net_struct(model)
-        st = _st(dev)
-        for k0 in range(0, N, B):
-            m = min(B, N - k0)
-            _lib.check(L.ngp_points_rays(V, HW, 1, k0, m, poses.data_ptr(), directions.data_ptr(), idx[0].data_ptr(),
-                                         idx[1].data_ptr(), o.data_ptr(), d.data_ptr(), st), "ngp_points_rays")
-            if m < B:  # the last chunk's spare rays start behind the box and leave it: they never march
-                o[m:] = torch.tensor([c[0], c[1], c[2] + 2 * h[2] + 1.0], device=dev)
-                d[m:] = torch.tensor([0.0, 0.0, 1.0], device=dev)
-            _lib.check(L.ngp_render_infer_frame(C.byref(net), C.byref(cfg), o.data_ptr(), d.data_ptr(),
-                                                model.density_bitfield.data_ptr(), opacity[k0:].data_ptr(),
-                                                depth[k0:].data_ptr(), rgb[k0:].data_ptr(), total.data_ptr(), ws.data_ptr(),
-                                                ws.numel(), st), "ngp_render_infer_frame")
-        del ws
+        for _ in _render_chunks(model, cfg, poses, directions, 1, N, lambda k0: (opacity[k0:], depth[k0:], rgb[k0:])):
+            pass
     return {"opacity": opacity[:N].view(V, HW), "depth": depth[:N].view(V, HW), "rgb": rgb[:N].view(V, HW, 3)}
 
 

@@ -17,6 +17,27 @@ MAX_SAMPLES = 1024
 NEAR_DISTANCE = 0.01
 
 
+def default_exp_step_factor(model):
+    """train.py's rule, read from the model: 1/256 (exponential steps) for scale > 0.5, else 0 (constant steps)"""
+    return 1 / 256 if float(model.scale) > 0.5 else 0.0
+
+
+def infer_cfg(model, n_rays, exp_step_factor, bg, T_threshold=1e-4, sample_budget=MAX_SAMPLES):
+    """NgpInferCfg of the inference wavefront for n_rays rays of model: the marcher's MAX_SAMPLES step bound, the near
+    plane NEAR_DISTANCE, background bg in all three channels, the outer loop's sample_budget and per-round sample
+    buffers of max(4 n_rays, 2^16), so the per-ray quota is never clipped"""
+    cfg = _lib.NgpInferCfg()
+    cfg.n_rays, cfg.cascades, cfg.grid_size, cfg.max_samples = n_rays, model.cascades, model.grid_size, MAX_SAMPLES
+    cfg.scale, cfg.exp_step_factor = float(model.scale), float(exp_step_factor)
+    cfg.T_threshold, cfg.near_distance = float(T_threshold), NEAR_DISTANCE
+    c, h = model.center.flatten().tolist(), model.half_size.flatten().tolist()
+    for k in range(3):
+        cfg.center[k], cfg.half_size[k], cfg.bg[k] = c[k], h[k], bg
+    cfg.sample_budget = int(sample_budget)
+    cfg.max_round_samples = max(4 * n_rays, 1 << 16)
+    return cfg
+
+
 @torch.amp.autocast('cuda')
 def render(model, rays_o, rays_d, **kwargs):
     rays_o = rays_o.contiguous()
@@ -63,16 +84,8 @@ def _render_rays_test_fused(model, rays_o, rays_d, hits_t, **kwargs):
     dev = rays_o.device
     with torch.cuda.device(dev):
         L = _lib.lib()
-        cfg = _lib.NgpInferCfg()
-        cfg.n_rays, cfg.cascades, cfg.grid_size, cfg.max_samples = N, model.cascades, model.grid_size, MAX_SAMPLES
-        cfg.scale, cfg.exp_step_factor = float(model.scale), float(exp_step_factor)
-        cfg.T_threshold, cfg.near_distance = float(kwargs.get('T_threshold', 1e-4)), NEAR_DISTANCE
-        c, h = model.center.flatten().tolist(), model.half_size.flatten().tolist()
-        bg = 1.0 if exp_step_factor == 0 else 0.0
-        for k in range(3):
-            cfg.center[k], cfg.half_size[k], cfg.bg[k] = c[k], h[k], bg
-        cfg.sample_budget = int(kwargs.get('max_samples', MAX_SAMPLES))
-        cfg.max_round_samples = max(4 * N, 1 << 16)
+        cfg = infer_cfg(model, N, exp_step_factor, 1.0 if exp_step_factor == 0 else 0.0, kwargs.get('T_threshold', 1e-4),
+                        kwargs.get('max_samples', MAX_SAMPLES))
         ws_bytes = L.ngp_render_infer_workspace(N, cfg.max_round_samples)
         # persistent per-model buffers: workspace, staged rays and outputs keep their addresses from frame to frame, which
         # is what lets the cached frame graph be replayed

@@ -23,9 +23,9 @@ import numpy as np
 import torch
 
 from . import _lib
-from .mesh import _chk, _need, _st, _three, cluster_grid
+from .mesh import _chk, _need, _np, _st, _three, cluster_grid
 from .models.networks import _net_struct
-from .models.rendering import MAX_SAMPLES, NEAR_DISTANCE
+from .models.rendering import default_exp_step_factor, infer_cfg
 
 CHUNK = 1 << 18          # rays per render: the wavefront's buffers and its cached graph are reused from chunk to chunk
 MAX_RAYS = 1 << 28
@@ -78,6 +78,42 @@ def _k(nb_neighbors, fn):
     return int(nb_neighbors)
 
 
+def _render_chunks(model, cfg, poses, directions, step, n, maps, ev=None):
+    """Renders rays 0 .. n - 1, cfg.n_rays at a time: ray k through the global pixel (k step) mod (views * pixels) of
+    poses x directions (ngp_points_rays), then ngp_render_infer_frame into the (opacity, depth, rgb) tensors that
+    maps(k0) returns for the chunk starting at ray k0. Yields (k0, m, idx, o, d) once a chunk's render is enqueued: its
+    m rays' (view, pixel) ids, origins and directions, overwritten by the next chunk. ev: CUDA events recorded before
+    the rays, before the render and after it."""
+    dev, B, L = poses.device, cfg.n_rays, _lib.lib()
+    ws = torch.empty(L.ngp_render_infer_workspace(B, cfg.max_round_samples), device=dev, dtype=torch.uint8)
+    idx = torch.empty(2, B, device=dev, dtype=torch.int64)
+    o, d = torch.empty(B, 3, device=dev), torch.empty(B, 3, device=dev)
+    total = torch.zeros(1, device=dev, dtype=torch.int64)
+    c, h = model.center.flatten().tolist(), model.half_size.flatten().tolist()
+    net, keep = _net_struct(model)
+    st = _st(dev)
+    for k0 in range(0, n, B):
+        m = min(B, n - k0)
+        if ev:
+            ev[0].record()
+        _lib.check(L.ngp_points_rays(poses.shape[0], directions.shape[0], step, k0, m, poses.data_ptr(),
+                                     directions.data_ptr(), idx[0].data_ptr(), idx[1].data_ptr(), o.data_ptr(), d.data_ptr(),
+                                     st), "ngp_points_rays")
+        if m < B:  # the last chunk's spare rays start behind the box and leave it: they never march
+            o[m:] = torch.tensor([c[0], c[1], c[2] + 2 * h[2] + 1.0], device=dev)
+            d[m:] = torch.tensor([0.0, 0.0, 1.0], device=dev)
+        if ev:
+            ev[1].record()
+        opacity, depth, rgb = maps(k0)
+        _lib.check(L.ngp_render_infer_frame(C.byref(net), C.byref(cfg), o.data_ptr(), d.data_ptr(),
+                                            model.density_bitfield.data_ptr(), opacity.data_ptr(), depth.data_ptr(),
+                                            rgb.data_ptr(), total.data_ptr(), ws.data_ptr(), ws.numel(), st),
+                   "ngp_render_infer_frame")
+        if ev:
+            ev[2].record()
+        yield k0, m, idx, o, d
+
+
 @torch.no_grad()
 def extract_points(model, poses, directions, num_rays=1000000, min_opacity=0.5, bounds=None, exp_step_factor=None,
                    chunk=CHUNK, return_rays=False, timings=None):
@@ -120,33 +156,19 @@ def extract_points(model, poses, directions, num_rays=1000000, min_opacity=0.5, 
         raise RuntimeError("ngp_pl_b200.points.extract_points: bounds need lo <= hi on every axis, got %s .. %s" % (lo, hi))
     box = (C.c_float * 6)(*[float(x) for x in np.concatenate([lo, hi])])
     if exp_step_factor is None:
-        exp_step_factor = 1 / 256 if float(model.scale) > 0.5 else 0.0
+        exp_step_factor = default_exp_step_factor(model)
     N = n_views * n_pix
     R = min(int(num_rays), N)
-    g = golden_step(N)
     B = min(int(chunk), R)
     L = _lib.lib()
-
-    cfg = _lib.NgpInferCfg()
-    cfg.n_rays, cfg.cascades, cfg.grid_size, cfg.max_samples = B, model.cascades, model.grid_size, MAX_SAMPLES
-    cfg.scale, cfg.exp_step_factor = float(model.scale), float(exp_step_factor)
-    cfg.T_threshold, cfg.near_distance = 1e-4, NEAR_DISTANCE
-    c, h = model.center.flatten().tolist(), model.half_size.flatten().tolist()
-    for k in range(3):
-        cfg.center[k], cfg.half_size[k], cfg.bg[k] = c[k], h[k], 0.0
-    cfg.sample_budget = MAX_SAMPLES
-    cfg.max_round_samples = max(4 * B, 1 << 16)
+    cfg = infer_cfg(model, B, exp_step_factor, 0.0)
     with torch.cuda.device(dev):
         infer_bytes = L.ngp_render_infer_workspace(B, cfg.max_round_samples)
         pts_bytes = L.ngp_points_workspace(B)
         _need(dev, R * 27 + B * 72 + infer_bytes + pts_bytes + (R * 68 if return_rays else 0),
               "%d rays in chunks of %d" % (R, B), "extract_points")
-        ws = torch.empty(infer_bytes, device=dev, dtype=torch.uint8)
         pws = _ws(dev, B, "rays", "extract_points")
-        idx = torch.empty(2, B, device=dev, dtype=torch.int64)
-        o, d = torch.empty(B, 3, device=dev), torch.empty(B, 3, device=dev)
         opacity, depth, rgb = torch.empty(B, device=dev), torch.empty(B, device=dev), torch.empty(B, 3, device=dev)
-        total = torch.zeros(1, device=dev, dtype=torch.int64)
         out = _empty(dev, R)
         rays = None
         if return_rays:
@@ -154,29 +176,13 @@ def extract_points(model, poses, directions, num_rays=1000000, min_opacity=0.5, 
                     "rays_o": torch.empty(R, 3, device=dev), "rays_d": torch.empty(R, 3, device=dev),
                     "opacity": torch.empty(R, device=dev), "depth": torch.empty(R, device=dev),
                     "rgb": torch.empty(R, 3, device=dev)}
-        net, keep = _net_struct(model)
         st = _st(dev)
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)] if timings is not None else None
         acc = [0.0, 0.0, 0.0]
         n_out = 0
         cnt = C.c_int64()
-        for k0 in range(0, R, B):
-            m = min(B, R - k0)
-            if ev:
-                ev[0].record()
-            _lib.check(L.ngp_points_rays(n_views, n_pix, g, k0, m, poses.data_ptr(), directions.data_ptr(), idx[0].data_ptr(),
-                                         idx[1].data_ptr(), o.data_ptr(), d.data_ptr(), st), "ngp_points_rays")
-            if m < B:  # the last chunk's spare rays start behind the box and leave it: they never march
-                o[m:] = torch.tensor([c[0], c[1], c[2] + 2 * h[2] + 1.0], device=dev)
-                d[m:] = torch.tensor([0.0, 0.0, 1.0], device=dev)
-            if ev:
-                ev[1].record()
-            _lib.check(L.ngp_render_infer_frame(C.byref(net), C.byref(cfg), o.data_ptr(), d.data_ptr(),
-                                                model.density_bitfield.data_ptr(), opacity.data_ptr(), depth.data_ptr(),
-                                                rgb.data_ptr(), total.data_ptr(), ws.data_ptr(), ws.numel(), st),
-                       "ngp_render_infer_frame")
-            if ev:
-                ev[2].record()
+        for k0, m, idx, o, d in _render_chunks(model, cfg, poses, directions, golden_step(N), R,
+                                               lambda k0: (opacity, depth, rgb), ev):
             _lib.check(L.ngp_points_backproject(o.data_ptr(), d.data_ptr(), opacity.data_ptr(), depth.data_ptr(),
                                                 rgb.data_ptr(), m, float(min_opacity), box,
                                                 out["points"][n_out:].data_ptr(), out["colors"][n_out:].data_ptr(),
@@ -193,7 +199,7 @@ def extract_points(model, poses, directions, num_rays=1000000, min_opacity=0.5, 
                 for key, t in (("rays_o", o), ("rays_d", d), ("opacity", opacity), ("depth", depth), ("rgb", rgb)):
                     rays[key][k0:k0 + m] = t[:m]
             n_out += cnt.value
-        del ws, pws
+        del pws
     if timings is not None:
         for s, name in enumerate(("rays", "render", "backproject")):
             timings[name] = timings.get(name, 0.0) + acc[s]
@@ -202,10 +208,6 @@ def extract_points(model, poses, directions, num_rays=1000000, min_opacity=0.5, 
     if rays is not None:
         res.update(rays)
     return res
-
-
-def _np(a):
-    return a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
 
 
 @torch.no_grad()

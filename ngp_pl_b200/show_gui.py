@@ -100,7 +100,7 @@ class ViewRenderer:
     def __init__(self, model, K, img_wh, exp_step_factor, quality=90):
         import torch
         from . import _lib, datasets
-        from .models.rendering import MAX_SAMPLES, NEAR_DISTANCE
+        from .models.rendering import infer_cfg
         bits = getattr(model, "density_bitfield", None)
         if bits is None or not bits.is_cuda:
             raise RuntimeError("ngp_pl_b200.show_gui: the model must live on a CUDA device (there is no CPU path)")
@@ -111,17 +111,8 @@ class ViewRenderer:
         n = self.W * self.H
         self.n = n
         L = self._L = _lib.lib()
-        cfg = _lib.NgpInferCfg()
-        cfg.n_rays, cfg.cascades, cfg.grid_size, cfg.max_samples = n, model.cascades, model.grid_size, MAX_SAMPLES
-        cfg.scale, cfg.exp_step_factor = float(model.scale), float(exp_step_factor)
-        cfg.T_threshold, cfg.near_distance = T_THRESHOLD, NEAR_DISTANCE
-        c, h = model.center.flatten().tolist(), model.half_size.flatten().tolist()
-        bg = 1.0 if exp_step_factor == 0 else 0.0
-        for k in range(3):
-            cfg.center[k], cfg.half_size[k], cfg.bg[k] = c[k], h[k], bg
-        cfg.sample_budget = SAMPLE_BUDGET
-        cfg.max_round_samples = max(4 * n, 1 << 16)
-        self.cfg = cfg
+        self.cfg = cfg = infer_cfg(model, n, exp_step_factor, 1.0 if exp_step_factor == 0 else 0.0, T_THRESHOLD,
+                                   SAMPLE_BUDGET)
         self.views = {m: _lib.NgpViewCfg(k, int(quality), self.H, self.W) for m, k in MODES.items()}
         ws = L.ngp_render_view_workspace(C.byref(cfg), C.byref(self.views["rgb"]))
         cap = L.ngp_jpeg_capacity(self.H, self.W)

@@ -349,9 +349,9 @@ def preview(model, splats, poses, K, img_wh, directions, save_dir=None, exp_step
     (rgb * 255).astype(uint8), PNG-encoded on the device."""
     import os
     from . import images, metrics
-    from .models.rendering import render as render_model
+    from .models.rendering import default_exp_step_factor, render as render_model
     if exp_step_factor is None:
-        exp_step_factor = 1 / 256 if float(model.scale) > 0.5 else 0.0
+        exp_step_factor = default_exp_step_factor(model)
     bg = 1.0 if exp_step_factor == 0 else 0.0
     W, H = int(img_wh[0]), int(img_wh[1])
     dev = splats.device

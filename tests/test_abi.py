@@ -1,6 +1,6 @@
 """CPU-side checks of the drop-in boundary: libngp_b200.so loads, exports every symbol that
-include/ngp_b200.h declares (no compute calls without a GPU), the ctypes table agrees with the header,
-and the Python shim exposes the reference's twelve `vren` names."""
+include/ngp_b200.h declares (no compute calls without a GPU), the ctypes binding read from the header agrees with
+the C compiler and with bindings written out by hand, and the Python shim exposes the reference's twelve `vren` names."""
 import os
 import re
 
@@ -39,21 +39,99 @@ def test_header_is_plain_c():
         assert r.returncode == 0, r.stdout.decode()
 
 
-def test_struct_layouts_match_header():
-    """sizeof of the by-value structs as the C compiler sees them == ctypes mirrors"""
-    import ctypes, subprocess, tempfile
-    from ngp_pl_b200 import _lib
-    names = ["NgpGridMeta", "NgpNet", "NgpSamples", "NgpTrainCfg"]
-    present = [n for n in names if re.search(r"\}\s*%s\s*;" % n, open(HEADER).read())]
+def _probe(body):
+    """stdout of a C program that includes the header and runs `body` in main"""
+    import subprocess, tempfile
     with tempfile.TemporaryDirectory() as d:
         c = os.path.join(d, "t.c")
-        body = "".join('printf("%%zu\\n", sizeof(%s));' % n for n in present)
-        open(c, "w").write('#include <stdio.h>\n#include "ngp_b200.h"\nint main(void){%s return 0;}\n' % body)
+        open(c, "w").write('#include <stddef.h>\n#include <stdio.h>\n#include "ngp_b200.h"\n'
+                           'int main(void){%s return 0;}\n' % body)
         exe = os.path.join(d, "t")
         subprocess.check_call(["gcc", "-I", os.path.dirname(HEADER), c, "-o", exe])
-        sizes = [int(x) for x in subprocess.check_output([exe]).decode().split()]
-    for n, s in zip(present, sizes):
-        assert ctypes.sizeof(getattr(_lib, n)) == s, "%s: C says %d, ctypes says %d" % (n, s, ctypes.sizeof(getattr(_lib, n)))
+        return subprocess.check_output([exe]).decode().split()
+
+
+def test_struct_layouts_match_header():
+    """sizeof and the offsetof of every field of every struct, as the C compiler sees them == the ctypes mirrors"""
+    import ctypes
+    from ngp_pl_b200 import _lib
+    names = re.findall(r"\}\s*(Ngp\w+)\s*;", open(HEADER).read())
+    assert len(names) == 9
+    want, body = [], ""
+    for n in names:
+        cls = getattr(_lib, n)
+        want.append(("sizeof(%s)" % n, ctypes.sizeof(cls)))
+        body += 'printf("%%zu\\n", sizeof(%s));' % n
+        for f, _ in cls._fields_:
+            want.append(("%s.%s" % (n, f), getattr(cls, f).offset))
+            body += 'printf("%%zu\\n", offsetof(%s, %s));' % (n, f)
+    got = [int(x) for x in _probe(body)]
+    assert len(got) == len(want)
+    for (what, py), c in zip(want, got):
+        assert py == c, "%s: C says %d, ctypes says %d" % (what, c, py)
+
+
+def test_defines_match_header():
+    """every valued #define NGP_* is a constant of _lib with the value the C compiler gives it"""
+    from ngp_pl_b200 import _lib
+    names = re.findall(r"^#define[ \t]+(NGP_\w+)[ \t]+\S", open(HEADER).read(), re.M)
+    assert len(names) >= 50
+    got = _probe("".join('printf("%%.17g\\n", (double)(%s));' % n for n in names))
+    for n, v in zip(names, got):
+        assert getattr(_lib, n) == float(v), n
+    assert _lib.ABI_VERSION == _lib.NGP_ABI_VERSION == 15
+    assert _lib.NGP_INFER_FIELDS == ("t_cur", "t_end", "alive0", "alive1", "ray_start", "ray_n", "ray_idx", "ts", "deltas",
+                                     "sigmas", "rgbs", "counters")
+
+
+def test_bindings_read_from_header():
+    """a few bindings written out by hand, one per kind of type the header reader maps"""
+    import ctypes as C
+    from ngp_pl_b200 import _lib
+    S = _lib.SIGNATURES
+    assert S["ngp_grid_meta"] == (C.c_uint32, [C.c_int, C.c_int, C.c_int, C.c_float, C.POINTER(_lib.NgpGridMeta)])
+    assert S["ngp_launch_count"] == (C.c_ulonglong, [])
+    assert S["ngp_splat_fit"][1][7] is C.c_double
+    assert S["ngp_adam_step_fused"][1][5:7] == [C.c_uint64, C.c_uint64]
+    assert S["ngp_render_infer_workspace"] == (C.c_size_t, [C.c_int, C.c_int64])
+    assert S["ngp_render_train_fwd"][1][:3] == [C.POINTER(_lib.NgpNet), C.POINTER(_lib.NgpTrainCfg),
+                                                C.POINTER(_lib.NgpTrainBuffers)]
+    assert S["ngp_packbits"][1][0] is C.c_void_p and S["ngp_cast_params"][1][1] is C.c_void_p
+    meta = dict(_lib.NgpGridMeta._fields_)
+    assert meta["offset"]._type_ is C.c_uint32 and meta["offset"]._length_ == 17 and meta["scale"]._type_ is C.c_float
+    assert _lib.NgpTrainCfg._fields_[:8] == [("n_rays", C.c_int32), ("cascades", C.c_int32), ("grid_size", C.c_int32),
+                                             ("max_samples", C.c_int32), ("scale", C.c_float),
+                                             ("exp_step_factor", C.c_float), ("T_threshold", C.c_float),
+                                             ("near_distance", C.c_float)]
+    assert [(f, t._length_) for f, t in _lib.NgpTrainCfg._fields_[8:11]] == [("center", 3), ("half_size", 3), ("bg", 3)]
+    assert dict(_lib.NgpNet._fields_)["meta"] is _lib.NgpGridMeta
+    assert dict(_lib.NgpNet._fields_)["enc_params_h"] is C.c_void_p
+
+
+@pytest.mark.parametrize("decl, named", [
+    ("int ngp_bad(long n, void* stream);", "ngp_bad"),
+    ("typedef struct {\n    int32_t a;\n    long b;\n} NgpBad;", "NgpBad.b"),
+    ("#define NGP_BAD (1 * 2)", "NGP_BAD"),
+    ("#define NGP_BAD NGP_UNDEFINED", "NGP_BAD"),
+    ("int ngp_bad(int a[4]);", "ngp_bad"),
+])
+def test_header_reader_refuses_what_it_cannot_map(tmp_path, decl, named):
+    import ctypes as C
+    from ngp_pl_b200 import _lib
+    h = tmp_path / "bad.h"
+    good = "#define NGP_ONE 1\n/* a comment */\nint ngp_ok(int n, void* stream);\n"
+    h.write_text(good)
+    assert _lib.parse_header(str(h)) == ({"NGP_ONE": 1}, {}, {"ngp_ok": (C.c_int, [C.c_int, C.c_void_p])})
+    h.write_text(good + decl + "\n")
+    with pytest.raises(RuntimeError, match=re.escape(named)) as e:
+        _lib.parse_header(str(h))
+    assert str(h) in str(e.value)
+
+
+def test_header_reader_names_an_unreadable_header(tmp_path):
+    from ngp_pl_b200 import _lib
+    with pytest.raises(RuntimeError, match=re.escape(str(tmp_path / "missing.h"))):
+        _lib.parse_header(str(tmp_path / "missing.h"))
 
 
 def test_vren_surface():
